@@ -1,13 +1,10 @@
-// C ABI of libquda_b200.so (declared in include/b200_dslash.h).  Plain pointers and sizes only.
+// C ABI of libquda_b200.so (declared in include/b200_dslash.h).  Plain pointers and sizes only.  The Dslash, pack,
+// clover and twist entry points forward to plan.h's templates, with the CUDA launchers as their executor.
 #include <atomic>
 #include <cstdlib>
 #include <cstring>
 
-#include "launch.h"
-
-#ifndef B2_TMA_DEFAULT
-#define B2_TMA_DEFAULT 0
-#endif
+#include "plan.h"
 
 namespace b200
 {
@@ -43,22 +40,17 @@ namespace b200
     return 0;
   }
 
-  // B200_TMA=0|1|2 selects the TMA-staged marching kernel (2: fail instead of falling back when a shape is not served);
-  // B200_TMA_TILE="ty tz", B200_TMA_GRID, B200_TMA_LINKS (n shared-memory stages, -1 register
-  // stream), B200_TMA_L2PF (L2 prefetch look-ahead in items, -1 off), B200_TMA_PREFETCH, B200_TMA_RINGS="centre halo" tune it.  Read on every call (a handful of getenv lookups) so
-  // that tests and tuning scripts can switch between calls.
-  static void tma_knobs(LaunchRequest &rq)
-  {
-    const char *e = getenv("B200_TMA");
-    rq.tma = e ? atoi(e) : B2_TMA_DEFAULT;
-    if (!rq.tma) return;
-    if ((e = getenv("B200_TMA_TILE"))) sscanf(e, "%d %d", &rq.tma_ty, &rq.tma_tz);
-    if ((e = getenv("B200_TMA_GRID"))) rq.tma_grid = atoi(e);
-    if ((e = getenv("B200_TMA_LINKS"))) rq.tma_link_slots = atoi(e);
-    if ((e = getenv("B200_TMA_PREFETCH"))) rq.tma_prefetch = atoi(e);
-    if ((e = getenv("B200_TMA_L2PF"))) rq.tma_l2_prefetch = atoi(e);
-    if ((e = getenv("B200_TMA_RINGS"))) sscanf(e, "%d %d", &rq.tma_center_slots, &rq.tma_halo_slots);
-  }
+  // the executor of plan.h's entry points: the per-precision CUDA launchers (inst_*.cu)
+  struct Cuda {
+    static int require_device() { return b200::require_device(); }
+    template <class P> static int dslash(const LaunchRequest &rq) { return launch_precision<P>(rq); }
+    template <class P> static int tma(const LaunchRequest &rq) { return launch_tma_precision<P>(rq); }
+    template <class P> static int mrhs(const MrhsRequest &rq) { return launch_mrhs_precision<P>(rq); }
+    template <class P> static int clover(const CloverRequest &rq) { return launch_clover_precision<P>(rq); }
+    template <class P> static int twist(const TwistRequest &rq) { return launch_twist_precision<P>(rq); }
+    template <class P> static int pack(const PackRequest &rq) { return launch_pack_precision<P>(rq); }
+    template <class P> static int pack_multi(const PackRequest &rq, const PackBatchRequest &b) { return launch_pack_multi_precision<P>(rq, b); }
+  };
 
 } // namespace b200
 
@@ -76,131 +68,24 @@ size_t b200_ghost_face_bytes(int precision, const int X[4], int dim)
   return 2 * ghost_parity_bytes(precision, X, dim);
 }
 
-int b200_dslash_apply(const b200_dslash_args *a)
-{
-  if (int rc = require_device()) return rc;
-  LaunchRequest rq;
-  bool nothing_to_do = false;
-  if (int rc = make_request(rq, a, nothing_to_do)) return rc;
-  if (nothing_to_do) return B200_SUCCESS;
-  tma_knobs(rq);
-  if (rq.tma && rq.kernel == B200_KERNEL_AUTO && a->precision != B200_HALF) {
-    // TMA-staged marching kernel (tma_kernel.cuh) for the shapes it serves; anything else falls through
-    const int rc = a->precision == B200_DOUBLE ? launch_tma_precision<PrecF64>(rq) : launch_tma_precision<PrecF32>(rq);
-    if (rc != kTmaSkip) return rc;
-    if (rq.tma > 1) return set_error(B200_ERR_UNSUPPORTED, "B200_TMA=2: shape not served by the TMA kernel");
-  }
-  switch (a->precision) {
-  case B200_DOUBLE: return launch_precision<PrecF64>(rq);
-  case B200_SINGLE: return launch_precision<PrecF32>(rq);
-  case B200_HALF: return launch_precision<PrecH16>(rq);
-  }
-  return set_error(B200_ERR_INVALID, "precision %d not in {8,4,2}", a->precision);
-}
+int b200_dslash_apply(const b200_dslash_args *a) { return apply_dslash<Cuda>(a); }
 
 int b200_dslash_apply_multi(const b200_dslash_args *a, int n_src, const b200_spinor *out, const b200_spinor *in,
                             const b200_spinor *x)
 {
-  if (int rc = require_device()) return rc;
-  MrhsRequest rq;
-  bool batched = false;
-  if (int rc = make_mrhs_request(rq, a, n_src, out, in, x, batched)) return rc;
-  if (!batched) { // other kernel selectors / operators: source by source, each on its own ghost slab
-    for (int i = 0; i < n_src; i++) {
-      const b200_dslash_args one = source_args(*a, i, out, in, x);
-      if (int rc = b200_dslash_apply(&one)) return rc;
-    }
-    return B200_SUCCESS;
-  }
-  if (rq.interior_box && a->kernel == B200_KERNEL_AUTO) {
-    // partitioned lattice, whole operator: the boundary tiles of every source (they wait for the batch's arrival counters
-    // and read the source's own ghost slab) after the batched interior below -- the order the single-source AUTO path uses
-    b200_dslash_args interior = *a;
-    interior.kernel = B200_KERNEL_INTERIOR_TILES;
-    if (int rc = b200_dslash_apply_multi(&interior, n_src, out, in, x)) return rc;
-    for (int i = 0; i < n_src; i++) {
-      b200_dslash_args one = source_args(*a, i, out, in, x);
-      one.kernel = B200_KERNEL_BOUNDARY_TILES;
-      if (int rc = b200_dslash_apply(&one)) return rc;
-    }
-    return B200_SUCCESS;
-  }
-  // tuning knobs (defaults are the measured best): B200_MRHS_MODE=thread|cta|auto, B200_MRHS_BATCH (sources per thread),
-  // B200_MRHS_CTA_SOURCES (sources per CTA), B200_MRHS_L1=0|1 (link loads allocate in L1)
-  if (const char *e = getenv("B200_MRHS_MODE")) rq.mode = (strcmp(e, "cta") == 0) ? 1 : (strcmp(e, "thread") == 0 ? 0 : -1);
-  if (const char *e = getenv("B200_MRHS_BATCH")) rq.max_batch = atoi(e);
-  if (const char *e = getenv("B200_MRHS_CTA_SOURCES")) rq.cta_sources = atoi(e);
-  if (const char *e = getenv("B200_MRHS_L1")) rq.l1_links = atoi(e) ? 1 : 0;
-  if (const char *e = getenv("B200_MRHS_CTA_CFG")) rq.cta_cfg = atoi(e);
-  switch (a->precision) {
-  case B200_DOUBLE: return launch_mrhs_precision<PrecF64>(rq);
-  case B200_SINGLE: return launch_mrhs_precision<PrecF32>(rq);
-  case B200_HALF: return launch_mrhs_precision<PrecH16>(rq);
-  }
-  return set_error(B200_ERR_INVALID, "precision %d not in {8,4,2}", a->precision);
+  return apply_dslash_multi<Cuda>(a, n_src, out, in, x);
 }
 
 int b200_clover_apply(const b200_spinor *out, const b200_spinor *in, const b200_clover *A, int precision, int inverse,
                       int parity, void *stream)
 {
-  if (!out || !in || !A || !out->v || !in->v || !A->clover) return set_error(B200_ERR_INVALID, "null argument");
-  if (int rc = require_device()) return rc;
-  if (out->n_parity != 1 || in->n_parity != 1) return set_error(B200_ERR_INVALID, "ApplyClover acts on single-parity fields");
-  if (parity != 0 && parity != 1) return set_error(B200_ERR_INVALID, "parity %d", parity);
-  // inverse with a static-inverse build: the caller passes the A^-1 field and the kernel multiplies (same path as a
-  // forward apply); with dynamic_inverse the field holds A and the kernel solves by Cholesky
-  CloverRequest rq;
-  rq.out = out->v;
-  rq.out_norm = out->norm;
-  rq.in = in->v;
-  rq.in_norm = in->norm;
-  rq.A = *A;
-  rq.volume_cb = out->volume_cb;
-  rq.inverse = inverse ? 1 : 0;
-  rq.parity = parity;
-  rq.stream = stream;
-  switch (precision) {
-  case B200_DOUBLE: return launch_clover_precision<PrecF64>(rq);
-  case B200_SINGLE: return launch_clover_precision<PrecF32>(rq);
-  case B200_HALF: return launch_clover_precision<PrecH16>(rq);
-  }
-  return set_error(B200_ERR_INVALID, "precision %d not in {8,4,2}", precision);
-}
-
-// a, b of out = a (1 + i b gamma5) in for the singlet twist (dslash_gamma_helper.cuh:55-62)
-static void twist_coefficients(double &a, double &b, double kappa, double mu, int dagger, int inverse)
-{
-  if (!inverse) {
-    b = 2.0 * kappa * mu;
-    a = 1.0;
-  } else {
-    b = -2.0 * kappa * mu;
-    a = 1.0 / (1.0 + b * b);
-  }
-  if (dagger) b = -b;
+  return clover_apply<Cuda>(out, in, A, precision, inverse, parity, stream);
 }
 
 int b200_twist_gamma5(const b200_spinor *out, const b200_spinor *in, int precision, double kappa, double mu, int dagger,
                       int inverse, void *stream)
 {
-  if (!out || !in || !out->v || !in->v) return set_error(B200_ERR_INVALID, "b200_twist_gamma5: null argument");
-  if (int rc = require_device()) return rc;
-  if (out->n_parity != 1 || in->n_parity != 1 || out->volume_cb != in->volume_cb)
-    return set_error(B200_ERR_INVALID, "b200_twist_gamma5 acts on single-parity fields of equal volume");
-  TwistRequest rq;
-  rq.out = out->v;
-  rq.out_norm = out->norm;
-  rq.in = in->v;
-  rq.in_norm = in->norm;
-  rq.volume_cb = out->volume_cb;
-  twist_coefficients(rq.a, rq.b, kappa, mu, dagger, inverse);
-  rq.stream = stream;
-  switch (precision) {
-  case B200_DOUBLE: return launch_twist_precision<PrecF64>(rq);
-  case B200_SINGLE: return launch_twist_precision<PrecF32>(rq);
-  case B200_HALF: return launch_twist_precision<PrecH16>(rq);
-  }
-  return set_error(B200_ERR_INVALID, "precision %d not in {8,4,2}", precision);
+  return twist_gamma5<Cuda>(out, in, precision, kappa, mu, dagger, inverse, stream);
 }
 
 int b200_copy_spinor(const b200_spinor *native, int native_precision, void *host_order, int host_precision, int to_native,
@@ -311,97 +196,12 @@ int b200_comm_copy(void *dst, const void *src, size_t bytes)
   return check_cuda(cudaMemcpy(dst, src, bytes, cudaMemcpyDefault), "cudaMemcpy");
 }
 
-static int make_pack_request(PackRequest &rq, const b200_pack_args *a)
-{
-  if (!a || !a->in.v) return set_error(B200_ERR_INVALID, "null argument");
-  if (a->abi_version != B200_ABI_VERSION) return set_error(B200_ERR_INVALID, "ABI version mismatch");
-  memcpy(rq.X, a->X, sizeof(rq.X));
-  rq.parity = a->parity;
-  rq.dagger = a->dagger ? 1 : 0;
-  rq.in = a->in.v;
-  rq.in_norm = a->in.norm;
-  for (int d = 0; d < 4; d++) {
-    rq.comm_dim[d] = a->comm_dim[d];
-    for (int dir = 0; dir < 2; dir++) {
-      rq.dst[d][dir] = a->dst[d][dir];
-      rq.dst_norm[d][dir] = a->dst_norm[d][dir];
-      rq.signal[d][dir] = a->signal[d][dir];
-      if (a->comm_dim[d] && !a->dst[d][dir]) return set_error(B200_ERR_INVALID, "dst[%d][%d] is NULL", d, dir);
-    }
-  }
-  rq.block_counter = a->block_counter;
-  rq.seq = a->seq;
-  rq.stream = a->stream;
-  return 0;
-}
-
-int b200_pack_ghost(const b200_pack_args *a)
-{
-  PackRequest rq;
-  if (int rc = make_pack_request(rq, a)) return rc;
-  if (int rc = require_device()) return rc;
-  switch (a->precision) {
-  case B200_DOUBLE: return launch_pack_precision<PrecF64>(rq);
-  case B200_SINGLE: return launch_pack_precision<PrecF32>(rq);
-  case B200_HALF: return launch_pack_precision<PrecH16>(rq);
-  }
-  return set_error(B200_ERR_INVALID, "precision %d not in {8,4,2}", a->precision);
-}
+int b200_pack_ghost(const b200_pack_args *a) { return pack_ghost<Cuda>(a); }
 
 int b200_pack_ghost_multi(const b200_pack_args *a, int n_src, const b200_spinor *in, const size_t dst_stride[4])
 {
-  if (n_src < 1 || n_src > B200_MAX_MULTI_RHS) return set_error(B200_ERR_INVALID, "n_src %d not in [1, %d]", n_src, B200_MAX_MULTI_RHS);
-  if (!a || !in || !dst_stride) return set_error(B200_ERR_INVALID, "null argument");
-  b200_pack_args first = *a;
-  first.in = in[0];
-  PackRequest rq;
-  if (int rc = make_pack_request(rq, &first)) return rc;
-  PackBatchRequest batch {};
-  batch.n_src = n_src;
-  for (int s = 0; s < n_src; s++) {
-    if (!in[s].v) return set_error(B200_ERR_INVALID, "source %d is null", s);
-    if (in[s].n_parity != 1) return set_error(B200_ERR_INVALID, "the batched pack takes single-parity sources");
-    batch.in[s] = in[s].v;
-    batch.in_norm[s] = in[s].norm;
-  }
-  for (int d = 0; d < 4; d++) batch.dst_stride[d] = dst_stride[d];
-  if (int rc = check_src_stride("dst_stride", n_src, a->precision, a->X, a->comm_dim, dst_stride, 1)) return rc;
-  if (int rc = require_device()) return rc;
-  switch (a->precision) {
-  case B200_DOUBLE: return launch_pack_multi_precision<PrecF64>(rq, batch);
-  case B200_SINGLE: return launch_pack_multi_precision<PrecF32>(rq, batch);
-  case B200_HALF: return launch_pack_multi_precision<PrecH16>(rq, batch);
-  }
-  return set_error(B200_ERR_INVALID, "precision %d not in {8,4,2}", a->precision);
+  return pack_ghost_multi<Cuda>(a, n_src, in, dst_stride);
 }
 
-int b200_dslash_apply_fused(const b200_dslash_args *a, const b200_pack_args *p)
-{
-  if (int rc = require_device()) return rc;
-  LaunchRequest rq;
-  bool nothing_to_do = false;
-  if (int rc = make_request(rq, a, nothing_to_do)) return rc;
-  PackRequest pk;
-  if (int rc = make_pack_request(pk, p)) return rc;
-  if (a->kernel != B200_KERNEL_AUTO && a->kernel != B200_KERNEL_INTERIOR_TILES && a->kernel != B200_KERNEL_BOUNDARY_TILES)
-    return set_error(B200_ERR_INVALID, "fused Dslash: kernel must be AUTO (all roles), INTERIOR_TILES (interior role) or BOUNDARY_TILES (pack + boundary roles)");
-  if (p->in.v != a->in.v || p->precision != a->precision || p->parity != 1 - a->parity || (p->dagger != 0) != (a->dagger != 0))
-    return set_error(B200_ERR_INVALID, "pack arguments do not describe the faces of this Dslash's input");
-  if (a->out.n_parity != 1) return set_error(B200_ERR_INVALID, "the fused Dslash works on single-parity fields");
-  bool any = false;
-  for (int d = 0; d < 4; d++) {
-    if ((p->comm_dim[d] != 0) != (a->halo.comm_dim[d] != 0)) return set_error(B200_ERR_INVALID, "pack / halo partitioning differ in dimension %d", d);
-    if (p->X[d] != a->X[d]) return set_error(B200_ERR_INVALID, "pack / Dslash lattice extents differ");
-    any |= a->halo.comm_dim[d] != 0;
-  }
-  if (!any) return a->kernel == B200_KERNEL_BOUNDARY_TILES ? B200_SUCCESS : b200_dslash_apply(a); // nothing partitioned: the plain launch
-  if (a->halo.seq != p->seq) return set_error(B200_ERR_INVALID, "pack and halo carry different sequence numbers");
-  rq.fused_pack = &pk;
-  switch (a->precision) {
-  case B200_DOUBLE: return launch_precision<PrecF64>(rq);
-  case B200_SINGLE: return launch_precision<PrecF32>(rq);
-  case B200_HALF: return launch_precision<PrecH16>(rq);
-  }
-  return set_error(B200_ERR_INVALID, "precision %d not in {8,4,2}", a->precision);
-}
+int b200_dslash_apply_fused(const b200_dslash_args *a, const b200_pack_args *p) { return apply_dslash_fused<Cuda>(a, p); }
 }

@@ -1,4 +1,4 @@
-// __global__ wrappers around the site functions + the per-precision launch dispatcher.
+// __global__ wrappers around the site functions + the per-precision launchers that issue plan.h's launch plans.
 // One translation unit per storage precision includes this header (inst_f64.cu, inst_f32.cu, inst_h16.cu)
 // so the three compile in parallel.
 #pragma once
@@ -7,7 +7,7 @@
 #include <cuda_runtime.h>
 
 #include "dslash_site.h"
-#include "launch.h"
+#include "plan.h"
 
 namespace b200
 {
@@ -16,9 +16,6 @@ namespace b200
   // 64..128 threads: full x rows x a few y/z rows) and ptxas may use 65536 / (B2_MAXTILE * minBlocks) registers per
   // thread.  The stencil is latency bound (ncu: long-scoreboard stalls dominate), so registers spent on keeping the
   // loads of several hops in flight pay better than extra resident warps: fp64 255 regs, fp32 128, half 128.
-#ifndef B2_MAXTILE
-#define B2_MAXTILE 128
-#endif
 #ifndef B2_MINBLOCKS_F64
 #define B2_MINBLOCKS_F64 2
 #endif
@@ -28,7 +25,6 @@ namespace b200
 #ifndef B2_MINBLOCKS_H16
 #define B2_MINBLOCKS_H16 4
 #endif
-  constexpr int kMaxTile = B2_MAXTILE;
   template <class P> struct MinBlocks { static constexpr int value = B2_MINBLOCKS_F32; };
   template <> struct MinBlocks<PrecF64> { static constexpr int value = B2_MINBLOCKS_F64; };
   template <> struct MinBlocks<PrecH16> { static constexpr int value = B2_MINBLOCKS_H16; };
@@ -181,64 +177,20 @@ namespace b200
     out.save(v, x_cb);
   }
 
-  // Halo packing: one thread per (dim, face, face site); spin-project the boundary site and store the 12-real
-  // half spinor to the destination face buffer (local, or a peer GPU's ghost buffer mapped over NVLink).
-  // Face 0 (x[d] == 0) feeds the backward neighbour's forward hop, which uses P(d, dagger ? + : -);
-  // face 1 (x[d] == X[d]-1) feeds the forward neighbour's backward hop, P(d, dagger ? - : +).
-  // (reference: include/kernels/dslash_pack.cuh:134-200)
+  // Halo packing: one thread per (dim, face, face site) runs plan.h::pack_site, which stores the projected half spinor
+  // to the destination face buffer (local, or a peer GPU's ghost buffer mapped over NVLink).
 #ifndef B2_PACK_REMOTE_ADD
 #define B2_PACK_REMOTE_ADD 0
 #endif
-  template <class P> struct PackArgs {
-    Geom geom;
-    SpinorView<P> in;
-    GhostView<P> dst[4][2];
-    unsigned *signal[4][2]; // remote arrival flags (nullptr: none)
-    int *counter;           // 8 local block counters (zero between launches)
-    unsigned seq;
-    int comm_dim[4];
-    int parity;
-    int dagger;
-  };
-
-  // Which field a pack CTA reads and where its faces go: the launch's own (single exchange) ...
-  template <class P> struct PackOwnViews {
-    const PackArgs<P> &arg;
-    __device__ __forceinline__ const SpinorView<P> &in() const { return arg.in; }
-    __device__ __forceinline__ const GhostView<P> &dst(int d, int face) const { return arg.dst[d][face]; }
-  };
-  // ... or those of one source of a multi-RHS batch (pack_multi_kernel)
-  template <class P> struct PackSourceViews {
-    SpinorView<P> in_;
-    GhostView<P> dst_;
-    __device__ __forceinline__ const SpinorView<P> &in() const { return in_; }
-    __device__ __forceinline__ const GhostView<P> &dst(int, int) const { return dst_; }
-  };
-
   // one CTA of the pack: sites [blk * blockDim.x, ...) of face `face_id` = 2*d + face; `nblk` CTAs (of all sources of a
   // batch together) work on this face before its arrival counter moves
   template <class P, class Views>
   __device__ __forceinline__ void pack_block(const PackArgs<P> &arg, const Views &vw, int face_id, int blk, int nblk)
   {
-    using real = typename P::real;
     const Geom &g = arg.geom;
     const int d = face_id >> 1, face = face_id & 1;
     const int idx = blk * blockDim.x + threadIdx.x;
-    if (idx < g.face_cb[d]) {
-      int x[4];
-      coords_from_face(x, g, d, face ? g.X[d] - 1 : 0, idx, arg.parity);
-      const int x_cb = cb_from_coords(x, g);
-      const int sign = (face == 0) ? (arg.dagger ? +1 : -1) : (arg.dagger ? -1 : +1);
-      real v[24], h[12];
-      vw.in().load(v, x_cb);
-      switch (d) {
-      case 0: project(h, v, 0, sign); break;
-      case 1: project(h, v, 1, sign); break;
-      case 2: project(h, v, 2, sign); break;
-      default: project(h, v, 3, sign); break;
-      }
-      vw.dst(d, face).save(h, idx);
-    }
+    if (idx < g.face_cb[d]) pack_site(arg, vw, d, face, idx);
     unsigned *sig = arg.signal[d][face];
     if (sig) {
       // Arrival protocol: the flag word in the RECEIVER's memory holds the number of face sites that have landed in this
@@ -288,13 +240,6 @@ namespace b200
   // first source's slab.  The tickets count the CTAs of all sources, so the counter in the receiver's memory moves -- to
   // the same value as for a single exchange `seq` -- only when the last source's last site has landed; each source's
   // boundary kernel then waits on that one counter and reads its own slab.
-  template <class P> struct PackBatch {
-    typename P::store *in[B200_MAX_MULTI_RHS];
-    float *in_norm[B200_MAX_MULTI_RHS];
-    size_t dst_stride[4];
-    int n_src;
-  };
-
   template <class P>
   __global__ void __launch_bounds__(128) pack_multi_kernel(const __grid_constant__ PackArgs<P> arg, const __grid_constant__ PackBatch<P> batch)
   {
@@ -323,14 +268,9 @@ namespace b200
   //                               behind the first ~70 % of the interior CTAs (B200_FUSED_BOUNDARY_AT) and in front of the
   //                               rest, so their wait + latency is covered by interior work instead of forming a tail
   // Blocks are dispatched in index order, so the faces leave first and the interior streams while they fly.  No second
-  // stream, no events, no exterior read-modify-write pass.
-  struct FusedShape {
-    int n_pack, n_interior, n_boundary;
-    int n_interior_first; // interior CTAs dispatched before the boundary CTAs (the rest follow them)
-    int pack_start[9];    // prefix sums of the pack CTAs per face id
-    int gx, gy;           // interior tile grid (gz implied)
-  };
-
+  // stream, no events, no exterior read-modify-write pass.  The host twin decodes block indices with plan.h's
+  // fused_pack_face / fused_interior_tile / fused_tile_block; calling them here changes this kernel's machine code, so
+  // it keeps its own copy of the decode -- change both together.
   template <class P, int recon, bool dagger, bool xpay, OpType op>
   __global__ void __launch_bounds__(kMaxTile, MinBlocks<P>::value)
     dslash_fused_kernel(const __grid_constant__ DslashArgs<P, recon> arg, const __grid_constant__ TileMap tm,
@@ -580,166 +520,40 @@ namespace b200
     return check_cuda(cudaGetLastError(), "copy_clover launch");
   }
 
-  template <class P> int fill_pack_args(PackArgs<P> &arg, const PackRequest &rq)
-  {
-    geom_init(arg.geom, rq.X);
-    fill_spinor(arg.in, rq.in, rq.in_norm, arg.geom.volume_cb);
-    arg.parity = rq.parity;
-    arg.dagger = rq.dagger;
-    arg.counter = rq.block_counter;
-    arg.seq = rq.seq;
-    for (int d = 0; d < 4; d++) {
-      arg.comm_dim[d] = rq.comm_dim[d] ? 1 : 0;
-      for (int dir = 0; dir < 2; dir++) {
-        fill_ghost(arg.dst[d][dir], rq.dst[d][dir], rq.dst_norm[d][dir], arg.geom.face_cb[d]);
-        arg.signal[d][dir] = arg.comm_dim[d] ? reinterpret_cast<unsigned *>(rq.signal[d][dir]) : nullptr;
-      }
-    }
-    return 0;
-  }
-
-  // ------------------------------------------------------------------ host-side dispatch for one precision
+  // ------------------------------------------------------------------ host side: issue the launch plan of one request
   template <class P, int recon, bool dagger, bool xpay, OpType op>
-  int launch_config(const LaunchRequest &rq, const DslashArgs<P, recon> &arg)
+  int launch_config(OpCfg<dagger, xpay, op>, const LaunchRequest &rq, const DslashArgs<P, recon> &arg)
   {
+    LaunchPlan pl;
+    if (int rc = plan_dslash(pl, rq, arg)) return rc;
     cudaStream_t s = (cudaStream_t)rq.stream;
-    TileMap tm;
-    int threads, gx, gy, gz, rc;
-    if (int e = make_tile_map(tm, threads, rq.tile, arg.geom, kMaxTile)) return e;
-    const bool partitioned = arg.threads_ext[4] > 0;
-    const bool tiles_path = rq.kernel == B200_KERNEL_AUTO || rq.kernel == B200_KERNEL_INTERIOR_TILES || rq.kernel == B200_KERNEL_BOUNDARY_TILES
-      || rq.kernel == B200_KERNEL_INTERIOR_SITES || rq.kernel == B200_KERNEL_BOUNDARY_SITES;
-    if (tiles_path && !partitioned && (rq.kernel == B200_KERNEL_BOUNDARY_TILES || rq.kernel == B200_KERNEL_BOUNDARY_SITES)) return B200_SUCCESS;
-    if (partitioned && arg.n_parity == 1 && (rq.kernel == B200_KERNEL_INTERIOR_SITES || rq.kernel == B200_KERNEL_BOUNDARY_SITES)) {
-      // the interior / boundary role of the fused kernel alone (1-site-thick shells, no pack role): what a caller with its
-      // own pack launch puts on its main / side stream
-      PackArgs<P> pk {};
-      FusedShape fs {};
-      if (!box_grid(tm, arg.n_parity, gx, gy, gz, rc)) return rc ? rc : set_error(B200_ERR_INVALID, "empty lattice");
-      fs.gx = gx;
-      fs.gy = gy;
-      fs.n_interior = rq.kernel == B200_KERNEL_INTERIOR_SITES ? gx * gy * gz : 0;
-      fs.n_boundary = rq.kernel == B200_KERNEL_BOUNDARY_SITES ? (arg.threads_ext[4] + threads - 1) / threads : 0;
-      fs.n_interior_first = fs.n_interior;
-      dslash_fused_kernel<P, recon, dagger, xpay, op><<<fs.n_interior + fs.n_boundary, threads, 0, s>>>(arg, tm, pk, fs);
-      count_launch();
-      return check_cuda(cudaGetLastError(), "dslash launch");
-    }
-    if (partitioned && rq.fused_pack && arg.n_parity == 1
-        && (rq.kernel == B200_KERNEL_AUTO || rq.kernel == B200_KERNEL_INTERIOR_TILES || rq.kernel == B200_KERNEL_BOUNDARY_TILES)) {
-      // roles of this launch: AUTO = pack | interior | boundary in one grid; INTERIOR_TILES = the interior role alone
-      // (halo independent); BOUNDARY_TILES = pack | boundary (what a caller puts on a high-priority side stream)
-      const bool do_pack = rq.kernel != B200_KERNEL_INTERIOR_TILES, do_int = rq.kernel != B200_KERNEL_BOUNDARY_TILES,
-                 do_bnd = rq.kernel != B200_KERNEL_INTERIOR_TILES;
-      // pack + interior + boundary in ONE launch (dslash_fused_kernel)
-      PackArgs<P> pk;
-      if (int e = fill_pack_args(pk, *rq.fused_pack)) return e;
-      if (!rq.fused_pack->block_counter) return set_error(B200_ERR_INVALID, "fused Dslash needs the pack block_counter scratch");
-      FusedShape fs;
-      fs.pack_start[0] = 0;
-      for (int f = 0; f < 8; f++) {
-        const int d = f >> 1;
-        const int nblk = (do_pack && pk.comm_dim[d]) ? (arg.geom.face_cb[d] + threads - 1) / threads : 0;
-        fs.pack_start[f + 1] = fs.pack_start[f] + nblk;
+    for (int i = 0; i < pl.n; i++) {
+      const LaunchStep &l = pl.step[i];
+      const dim3 grid(l.grid[0], l.grid[1], l.grid[2]);
+      switch (l.kind) {
+      case LAUNCH_INTERIOR:
+        if (l.masked)
+          dslash_interior_kernel<P, recon, dagger, xpay, op, true><<<grid, l.threads, 0, s>>>(arg, l.tm);
+        else
+          dslash_interior_kernel<P, recon, dagger, xpay, op, false><<<grid, l.threads, 0, s>>>(arg, l.tm);
+        break;
+      case LAUNCH_BOUNDARY: dslash_boundary_kernel<P, recon, dagger, xpay, op><<<grid, l.threads, 0, s>>>(arg, l.tm, l.st); break;
+      case LAUNCH_EXTERIOR: dslash_exterior_kernel<P, recon, dagger, xpay, op><<<grid, l.threads, 0, s>>>(arg); break;
+      case LAUNCH_FUSED: {
+        PackArgs<P> pk {};
+        if (rq.fused_pack) fill_pack_args(pk, *rq.fused_pack);
+        dslash_fused_kernel<P, recon, dagger, xpay, op><<<grid, l.threads, 0, s>>>(arg, l.tm, pk, l.fs);
+        break;
       }
-      fs.n_pack = fs.pack_start[8];
-      if (!box_grid(tm, arg.n_parity, gx, gy, gz, rc)) return rc ? rc : set_error(B200_ERR_INVALID, "empty lattice");
-      fs.gx = gx;
-      fs.gy = gy;
-      fs.n_interior = do_int ? gx * gy * gz : 0;
-      fs.n_boundary = do_bnd ? (arg.threads_ext[4] + threads - 1) / threads : 0;
-      static int boundary_at = -1; // percent of the interior CTAs dispatched before the boundary CTAs
-      if (boundary_at < 0) {
-        const char *e = getenv("B200_FUSED_BOUNDARY_AT");
-        boundary_at = e ? atoi(e) : 70;
-        if (boundary_at < 0 || boundary_at > 100) boundary_at = 100;
       }
-      fs.n_interior_first = (int)((long long)fs.n_interior * boundary_at / 100);
-      dslash_fused_kernel<P, recon, dagger, xpay, op><<<fs.n_pack + fs.n_interior + fs.n_boundary, threads, 0, s>>>(arg, tm, pk, fs);
-      count_launch();
-      return check_cuda(cudaGetLastError(), "fused dslash launch");
-    }
-    if (tiles_path && partitioned) {
-      // Tile schedule: tiles that touch no partitioned face run now (branch-free kernel, overlapping the halo that is
-      // in flight over NVLink); the boundary tiles follow in ONE launch that acquires the arrival flags and updates
-      // its sites completely -- no partial sums, no read-modify-write pass.
-      SlabTable st;
-      const int nb = split_boundary(tm, st, arg.comm_dim);
-      if (rq.kernel != B200_KERNEL_BOUNDARY_TILES) {
-        if (box_grid(tm, arg.n_parity, gx, gy, gz, rc)) {
-          dslash_interior_kernel<P, recon, dagger, xpay, op, false><<<dim3(gx, gy, gz), threads, 0, s>>>(arg, tm);
-          count_launch();
-        } else if (rc) {
-          return rc;
-        }
-      }
-      if (nb > 0 && rq.kernel != B200_KERNEL_INTERIOR_TILES) {
-        dslash_boundary_kernel<P, recon, dagger, xpay, op><<<dim3(nb, arg.n_parity, 1), threads, 0, s>>>(arg, tm, st);
-        count_launch();
-      }
-      return check_cuda(cudaGetLastError(), "dslash launch");
-    }
-    if (rq.kernel != B200_KERNEL_EXTERIOR) { // AUTO / INTERIOR_TILES on an unpartitioned lattice, or reference-style INTERIOR
-      if (!box_grid(tm, arg.n_parity, gx, gy, gz, rc)) return rc ? rc : set_error(B200_ERR_INVALID, "empty lattice");
-      dim3 grid(gx, gy, gz);
-      if (partitioned)
-        dslash_interior_kernel<P, recon, dagger, xpay, op, true><<<grid, threads, 0, s>>>(arg, tm);
-      else
-        dslash_interior_kernel<P, recon, dagger, xpay, op, false><<<grid, threads, 0, s>>>(arg, tm);
       count_launch();
     }
-    if (rq.kernel == B200_KERNEL_EXTERIOR && partitioned) {
-      dim3 grid((arg.threads_ext[4] + 127) / 128, arg.n_parity, 1);
-      dslash_exterior_kernel<P, recon, dagger, xpay, op><<<grid, 128, 0, s>>>(arg);
-      count_launch();
-    }
-    return check_cuda(cudaGetLastError(), "dslash launch");
-  }
-
-  template <class P, int recon> int launch_recon(const LaunchRequest &rq)
-  {
-    DslashArgs<P, recon> arg;
-    if (int rc = fill_args(arg, rq)) return rc;
-    const bool xp = rq.xpay, dg = rq.dagger;
-    switch (rq.op) {
-    case OP_WILSON:
-      if (dg)
-        return xp ? launch_config<P, recon, true, true, OP_WILSON>(rq, arg) :
-                    launch_config<P, recon, true, false, OP_WILSON>(rq, arg);
-      else
-        return xp ? launch_config<P, recon, false, true, OP_WILSON>(rq, arg) :
-                    launch_config<P, recon, false, false, OP_WILSON>(rq, arg);
-    case OP_CLOVER:
-      if (!xp) return set_error(B200_ERR_INVALID, "ApplyWilsonClover exists in xpay form only (a != 0)");
-      return dg ? launch_config<P, recon, true, true, OP_CLOVER>(rq, arg) :
-                  launch_config<P, recon, false, true, OP_CLOVER>(rq, arg);
-    case OP_CLOVER_PC:
-      if (dg)
-        return xp ? launch_config<P, recon, true, true, OP_CLOVER_PC>(rq, arg) :
-                    launch_config<P, recon, true, false, OP_CLOVER_PC>(rq, arg);
-      else
-        return xp ? launch_config<P, recon, false, true, OP_CLOVER_PC>(rq, arg) :
-                    launch_config<P, recon, false, false, OP_CLOVER_PC>(rq, arg);
-    case OP_TM: // xpay form only
-      return dg ? launch_config<P, recon, true, true, OP_TM>(rq, arg) : launch_config<P, recon, false, true, OP_TM>(rq, arg);
-    case OP_TM_PC:
-      if (dg && !rq.asymmetric) // symmetric dagger: the rotation acts on the neighbour spinors before the hop
-        return xp ? launch_config<P, recon, true, true, OP_TM_PC_PRE>(rq, arg) :
-                    launch_config<P, recon, true, false, OP_TM_PC_PRE>(rq, arg);
-      if (dg) return launch_config<P, recon, true, false, OP_TM_PC>(rq, arg); // asymmetric dagger (never xpay)
-      return xp ? launch_config<P, recon, false, true, OP_TM_PC>(rq, arg) : launch_config<P, recon, false, false, OP_TM_PC>(rq, arg);
-    }
-    return set_error(B200_ERR_INVALID, "unknown op %d", rq.op);
+    return check_cuda(cudaGetLastError(), rq.fused_pack ? "fused dslash launch" : "dslash launch");
   }
 
   template <class P> int launch_precision(const LaunchRequest &rq)
   {
-    switch (rq.reconstruct) {
-    case 18: return launch_recon<P, 18>(rq);
-    case 12: return launch_recon<P, 12>(rq);
-    case 8: return launch_recon<P, 8>(rq);
-    }
-    return set_error(B200_ERR_INVALID, "reconstruct %d not in {18,12,8}", rq.reconstruct);
+    return dispatch_dslash<P>(rq, [&](auto c, const auto &arg) { return launch_config(c, rq, arg); });
   }
 
   template <class P> int launch_clover_precision(const CloverRequest &rq)
@@ -772,45 +586,26 @@ namespace b200
 
   template <class P> int launch_pack_precision(const PackRequest &rq)
   {
+    int gx;
+    if (int rc = pack_blocks(gx, rq)) return rc;
+    if (!gx) return 0;
     PackArgs<P> arg;
-    if (int e = fill_pack_args(arg, rq)) return e;
-    int max_face = 0;
-    bool any_signal = false;
-    for (int d = 0; d < 4; d++) {
-      if (arg.comm_dim[d] && arg.geom.face_cb[d] > max_face) max_face = arg.geom.face_cb[d];
-      for (int dir = 0; dir < 2; dir++) any_signal |= (arg.signal[d][dir] != nullptr);
-    }
-    if (max_face == 0) return 0;
-    if (any_signal && !arg.counter) return set_error(B200_ERR_INVALID, "signal[] given without block_counter scratch");
-    dim3 grid((max_face + 127) / 128, 8, 1);
-    pack_kernel<P><<<grid, 128, 0, (cudaStream_t)rq.stream>>>(arg);
+    fill_pack_args(arg, rq);
+    pack_kernel<P><<<dim3(gx, 8, 1), 128, 0, (cudaStream_t)rq.stream>>>(arg);
     count_launch();
     return check_cuda(cudaGetLastError(), "pack launch");
   }
 
   template <class P> int launch_pack_multi_precision(const PackRequest &rq, const PackBatchRequest &b)
   {
+    int gx;
+    if (int rc = pack_blocks(gx, rq)) return rc;
+    if (!gx) return 0;
     PackArgs<P> arg;
-    if (int e = fill_pack_args(arg, rq)) return e;
-    PackBatch<P> batch {};
-    batch.n_src = b.n_src;
-    for (int s = 0; s < b.n_src; s++) {
-      SpinorView<P> v;
-      fill_spinor(v, b.in[s], b.in_norm[s], arg.geom.volume_cb);
-      batch.in[s] = v.v;
-      batch.in_norm[s] = v.norm;
-    }
-    int max_face = 0;
-    bool any_signal = false;
-    for (int d = 0; d < 4; d++) {
-      batch.dst_stride[d] = b.dst_stride[d];
-      if (arg.comm_dim[d] && arg.geom.face_cb[d] > max_face) max_face = arg.geom.face_cb[d];
-      for (int dir = 0; dir < 2; dir++) any_signal |= (arg.signal[d][dir] != nullptr);
-    }
-    if (max_face == 0) return 0;
-    if (any_signal && !arg.counter) return set_error(B200_ERR_INVALID, "signal[] given without block_counter scratch");
-    dim3 grid((max_face + 127) / 128, 8, b.n_src);
-    pack_multi_kernel<P><<<grid, 128, 0, (cudaStream_t)rq.stream>>>(arg, batch);
+    fill_pack_args(arg, rq);
+    PackBatch<P> batch;
+    fill_pack_batch(batch, b, arg.geom.volume_cb);
+    pack_multi_kernel<P><<<dim3(gx, 8, b.n_src), 128, 0, (cudaStream_t)rq.stream>>>(arg, batch);
     count_launch();
     return check_cuda(cudaGetLastError(), "batched pack launch");
   }

@@ -1,4 +1,4 @@
-// Multi-RHS (batched) Dslash: kernel wrapper + per-precision launcher.  The site code is dslash_site_mrhs
+// Multi-RHS (batched) Dslash: kernel wrappers + the per-precision launcher that issues plan.h's multi-RHS schedule.  The site code is dslash_site_mrhs
 // (dslash_site.h); one translation unit per storage precision includes this header (inst_mrhs_*.cu).
 //
 // Reference interface: the cvector_ref<ColorSpinorField> form of ApplyWilson / ApplyWilsonClover /
@@ -7,17 +7,12 @@
 #pragma once
 
 #include <cuda_runtime.h>
-#include <type_traits>
 
 #include "dslash_site.h"
-#include "launch.h"
+#include "plan.h"
 
 namespace b200
 {
-
-#ifndef B2_MAXTILE
-#define B2_MAXTILE 128
-#endif
 
   // Register budget: NS accumulators of 24 reals + the NS x 24-real spinor loads in flight.  2 CTAs of <= 128 threads
   // per SM gives ptxas the full 255 registers (fp64 NS = 2, fp32/half NS = 4); NS = 2 in fp32/half fits 168.
@@ -71,20 +66,17 @@ namespace b200
   }
 
   template <class P, int recon, bool dagger, bool xpay, OpType op>
-  int launch_mrhs_cta(const MrhsRequest &rq, const DslashArgs<P, recon> &arg)
+  int launch_mrhs_cta(OpCfg<dagger, xpay, op>, const MrhsRequest &rq, const DslashArgs<P, recon> &arg)
   {
     MrhsViews<P> f;
     fill_mrhs_views(f, rq);
-    TileMap tm;
-    int threads, gx, gy, gz, rc, nsb, n_batch;
-    if (int e = make_tile_map(tm, threads, rq.base.tile, arg.geom, B2_MAXTILE)) return e;
-    if (!mrhs_box(tm, rq, arg.comm_dim, arg.n_parity, gx, gy, gz, rc)) return rc;
-    mrhs_cta_shape(nsb, n_batch, rq.n_src, threads, B2_MAXTILE, rq.cta_sources);
-    if ((long long)gx * n_batch >= (1ll << 31)) return set_error(B200_ERR_INVALID, "lattice too large for the multi-RHS grid");
-    const dim3 grid(gx * n_batch, gy, gz), block(threads, nsb, 1);
+    MrhsGrid m;
+    if (int rc = plan_mrhs(m, rq, arg, true)) return rc;
+    if (!m.gx) return 0;
+    const dim3 grid(m.gx * m.n_batch, m.gy, m.gz), block(m.threads, m.nsb, 1);
     cudaStream_t st = (cudaStream_t)rq.base.stream;
 #define B2_CTA_LAUNCH(L1, CFG) \
-  dslash_mrhs_cta_kernel<P, recon, dagger, xpay, op, L1, CFG><<<grid, block, 0, st>>>(arg, f, tm, rq.n_src, n_batch)
+  dslash_mrhs_cta_kernel<P, recon, dagger, xpay, op, L1, CFG><<<grid, block, 0, st>>>(arg, f, m.tm, rq.n_src, m.n_batch)
     if (!rq.l1_links)
       B2_CTA_LAUNCH(false, 0);
     else if (rq.cta_cfg == 1)
@@ -98,86 +90,30 @@ namespace b200
     return check_cuda(cudaGetLastError(), "multi-RHS (CTA) dslash launch");
   }
 
-  template <class P, int recon, bool dagger, bool xpay, OpType op, int NS>
-  int launch_mrhs_batch(const MrhsRequest &rq, const DslashArgs<P, recon> &arg, int s0)
+  template <int NS, class P, int recon, bool dagger, bool xpay, OpType op>
+  int launch_mrhs_batch(OpCfg<dagger, xpay, op>, const MrhsRequest &rq, const DslashArgs<P, recon> &arg, int s0)
   {
     MrhsFields<P, NS> f;
     fill_mrhs_fields(f, rq, s0);
-    TileMap tm;
-    int threads, gx, gy, gz, rc;
-    if (int e = make_tile_map(tm, threads, rq.base.tile, arg.geom, B2_MAXTILE)) return e;
-    if (!mrhs_box(tm, rq, arg.comm_dim, arg.n_parity, gx, gy, gz, rc)) return rc;
-    dslash_mrhs_kernel<P, recon, dagger, xpay, op, NS><<<dim3(gx, gy, gz), threads, 0, (cudaStream_t)rq.base.stream>>>(arg, f, tm);
+    MrhsGrid m;
+    if (int rc = plan_mrhs(m, rq, arg, false)) return rc;
+    if (!m.gx) return 0;
+    dslash_mrhs_kernel<P, recon, dagger, xpay, op, NS><<<dim3(m.gx, m.gy, m.gz), m.threads, 0, (cudaStream_t)rq.base.stream>>>(arg, f, m.tm);
     count_launch();
     return check_cuda(cudaGetLastError(), "multi-RHS dslash launch");
   }
 
-  template <class P, int recon, bool dagger, bool xpay, OpType op>
-  int launch_mrhs_config(const MrhsRequest &rq, const DslashArgs<P, recon> &arg)
-  {
-    if (mrhs_mode(rq, P::bytes) == 1) return launch_mrhs_cta<P, recon, dagger, xpay, op>(rq, arg);
-    int s0 = 0;
-    while (s0 < rq.n_src) {
-      const int ns = mrhs_batch<P>(rq.n_src - s0, rq.max_batch);
-      int rc;
-      if constexpr (!std::is_same<P, PrecF64>::value) {
-        if (ns == 4) {
-          if ((rc = launch_mrhs_batch<P, recon, dagger, xpay, op, 4>(rq, arg, s0))) return rc;
-          s0 += 4;
-          continue;
-        }
-      }
-      if (ns >= 2) {
-        if ((rc = launch_mrhs_batch<P, recon, dagger, xpay, op, 2>(rq, arg, s0))) return rc;
-        s0 += 2;
-      } else { // odd one out: the single-source kernel (inst_*.cu)
-        LaunchRequest one = rq.base;
-        one.out = rq.out[s0];
-        one.in = rq.in[s0];
-        if (rq.base.xpay) one.x = rq.x[s0];
-        if ((rc = launch_precision<P>(one))) return rc;
-        s0 += 1;
-      }
-    }
-    return B200_SUCCESS;
-  }
-
-  template <class P, int recon> int launch_mrhs_recon(const MrhsRequest &rq)
-  {
-    DslashArgs<P, recon> arg;
-    if (int rc = fill_args(arg, rq.base)) return rc;
-    const bool xp = rq.base.xpay, dg = rq.base.dagger;
-    switch (rq.base.op) {
-    case OP_WILSON:
-      if (dg)
-        return xp ? launch_mrhs_config<P, recon, true, true, OP_WILSON>(rq, arg) :
-                    launch_mrhs_config<P, recon, true, false, OP_WILSON>(rq, arg);
-      else
-        return xp ? launch_mrhs_config<P, recon, false, true, OP_WILSON>(rq, arg) :
-                    launch_mrhs_config<P, recon, false, false, OP_WILSON>(rq, arg);
-    case OP_CLOVER:
-      if (!xp) return set_error(B200_ERR_INVALID, "ApplyWilsonClover exists in xpay form only (a != 0)");
-      return dg ? launch_mrhs_config<P, recon, true, true, OP_CLOVER>(rq, arg) :
-                  launch_mrhs_config<P, recon, false, true, OP_CLOVER>(rq, arg);
-    case OP_CLOVER_PC:
-      if (dg)
-        return xp ? launch_mrhs_config<P, recon, true, true, OP_CLOVER_PC>(rq, arg) :
-                    launch_mrhs_config<P, recon, true, false, OP_CLOVER_PC>(rq, arg);
-      else
-        return xp ? launch_mrhs_config<P, recon, false, true, OP_CLOVER_PC>(rq, arg) :
-                    launch_mrhs_config<P, recon, false, false, OP_CLOVER_PC>(rq, arg);
-    }
-    return set_error(B200_ERR_INVALID, "unknown op %d", rq.base.op);
-  }
-
   template <class P> int launch_mrhs_precision(const MrhsRequest &rq)
   {
-    switch (rq.base.reconstruct) {
-    case 18: return launch_mrhs_recon<P, 18>(rq);
-    case 12: return launch_mrhs_recon<P, 12>(rq);
-    case 8: return launch_mrhs_recon<P, 8>(rq);
-    }
-    return set_error(B200_ERR_INVALID, "reconstruct %d not in {18,12,8}", rq.base.reconstruct);
+    return dispatch_mrhs<P>(rq, [&](auto c, const auto &arg, auto ns, int s0) -> int {
+      constexpr int NS = decltype(ns)::value;
+      if constexpr (NS == 0)
+        return launch_mrhs_cta(c, rq, arg);
+      else if constexpr (NS == 1) // the odd one out: the single-source kernel (inst_*.cu)
+        return launch_precision<P>(mrhs_source(rq, s0));
+      else
+        return launch_mrhs_batch<NS>(c, rq, arg, s0);
+    });
   }
 
 } // namespace b200

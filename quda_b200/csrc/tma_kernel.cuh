@@ -5,7 +5,7 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 
-#include "launch.h"
+#include "plan.h"
 #include "tma.h"
 
 namespace b200
@@ -328,7 +328,7 @@ namespace b200
   }
 
   template <class P, int recon, bool dagger, bool xpay, OpType op>
-  int launch_tma(const LaunchRequest &rq, const DslashArgs<P, recon> &arg)
+  int launch_tma(OpCfg<dagger, xpay, op>, const LaunchRequest &rq, const DslashArgs<P, recon> &arg)
   {
     TmaPlan plan;
     TmaKnobs knobs {rq.tma_ty, rq.tma_tz, rq.tma_link_slots, rq.tma_center_slots, rq.tma_halo_slots, rq.tma_l2_prefetch};
@@ -344,8 +344,7 @@ namespace b200
         if (int rc = tma_encode(maps.m[pi][k], d[k])) return rc;
       }
     }
-    int grid = rq.tma_grid > 0 ? rq.tma_grid : tma_sm_count();
-    if (grid > plan.n_items) grid = plan.n_items;
+    const int grid = tma_grid(rq, plan.n_items, tma_sm_count());
     const int threads = (plan.n_cwarps + 1) * 32;
     cudaStream_t s = (cudaStream_t)rq.stream;
     auto go = [&](auto kern) -> int {
@@ -368,38 +367,9 @@ namespace b200
     return check_cuda(cudaGetLastError(), "dslash TMA launch");
   }
 
-  template <class P, int recon> int launch_tma_recon(const LaunchRequest &rq)
-  {
-    if constexpr (P::fixed) {
-      return kTmaSkip;
-    } else {
-      DslashArgs<P, recon> arg;
-      if (int rc = fill_args(arg, rq)) return rc;
-      if (arg.threads_ext[4] > 0) return kTmaSkip; // partitioned lattice: the halo schedule owns the launch
-      const bool xp = rq.xpay, dg = rq.dagger;
-      switch (rq.op) {
-      case OP_WILSON:
-        if (dg) return xp ? launch_tma<P, recon, true, true, OP_WILSON>(rq, arg) : launch_tma<P, recon, true, false, OP_WILSON>(rq, arg);
-        return xp ? launch_tma<P, recon, false, true, OP_WILSON>(rq, arg) : launch_tma<P, recon, false, false, OP_WILSON>(rq, arg);
-      case OP_CLOVER:
-        if (!xp) return kTmaSkip;
-        return dg ? launch_tma<P, recon, true, true, OP_CLOVER>(rq, arg) : launch_tma<P, recon, false, true, OP_CLOVER>(rq, arg);
-      case OP_CLOVER_PC:
-        if (dg) return xp ? kTmaSkip : launch_tma<P, recon, true, false, OP_CLOVER_PC>(rq, arg);
-        return xp ? launch_tma<P, recon, false, true, OP_CLOVER_PC>(rq, arg) : launch_tma<P, recon, false, false, OP_CLOVER_PC>(rq, arg);
-      }
-      return kTmaSkip;
-    }
-  }
-
   template <class P> int launch_tma_precision(const LaunchRequest &rq)
   {
-    switch (rq.reconstruct) {
-    case 18: return launch_tma_recon<P, 18>(rq);
-    case 12: return launch_tma_recon<P, 12>(rq);
-    case 8: return launch_tma_recon<P, 8>(rq);
-    }
-    return kTmaSkip;
+    return dispatch_tma<P>(rq, [&](auto c, const auto &arg) { return launch_tma(c, rq, arg); });
   }
 
 } // namespace b200

@@ -109,9 +109,10 @@ class Halo:
 
 
 def _apply(op, out, in_, U, a, x, parity, dagger, comm_override, A=None, halo=None, kernel=L.KERNEL_AUTO, tile=None,
-           stream=None, backend=None, b=0.0, asymmetric=False, fused_dst=None):
-    """`fused_dst` ([4][2] send targets as for PackGhost): run pack + interior + boundary as ONE launch
-    (b200_dslash_apply_fused) instead of a separate PackGhost call followed by the Dslash."""
+           stream=None, backend=None, b=0.0, asymmetric=False, fused_dst=None, block_counter=None):
+    """`fused_dst` ([4][2] send targets as for PackGhost) and `block_counter` (8 zeroed int32 of pack scratch): run
+    pack + interior + boundary as ONE launch (b200_dslash_apply_fused) instead of a separate PackGhost call followed by
+    the Dslash."""
     be = backend or cuda_backend()
     multi = isinstance(out, (list, tuple))  # the reference's cvector_ref batch: sources sharing U (and A)
     if multi:
@@ -155,6 +156,7 @@ def _apply(op, out, in_, U, a, x, parity, dagger, comm_override, A=None, halo=No
         p.parity, p.dagger = 1 - args.parity, args.dagger
         p.in_ = in_.desc()
         p.seq = args.halo.seq
+        p.block_counter = _ptr(block_counter)
         p.stream = stream
         be.call("dslash_apply_fused", C.byref(args), C.byref(p))
     else:

@@ -1,17 +1,16 @@
-// TEST-ONLY "host twin": runs the product's site code (quda_b200/csrc/dslash_site.h, core.h, clover.h --
-// the exact functions the CUDA kernels call) in plain CPU loops, through the same b200_dslash_args ABI and
-// the same argument validation (launch.h::make_request / fill_args).  It exists so that layouts, gauge
-// reconstruction, fixed-point handling, clover compression and the halo index maps can be checked against the
-// CPU oracle in the CPU-only test tier.  It is NOT part of the product: nothing under quda_b200/ loads it, and
-// libquda_b200.so has no CPU path.
+// TEST-ONLY "host twin": the library's entry points with a CPU executor.  Its twin_* functions forward to the same
+// templates as libquda_b200's b200_* functions (quda_b200/csrc/plan.h: argument validation, environment knobs,
+// orchestration, template dispatch and launch plans); the executor below walks every planned launch grid block by block
+// and thread by thread and runs the product's site code (dslash_site.h, core.h, clover.h -- the exact functions the CUDA
+// kernels call) in plain CPU loops.  It exists so that the launch logic, layouts, gauge reconstruction, fixed-point
+// handling, clover compression and the halo index maps can be checked against the CPU oracle in the CPU-only test tier.
+// It is NOT part of the product: nothing under quda_b200/ loads it, and libquda_b200.so has no CPU path.
 #include <cstdarg>
 #include <cstdio>
-#include <cstdlib>
 #include <numeric>
-#include <cstring>
 #include <vector>
 
-#include "../../quda_b200/csrc/launch.h"
+#include "../../quda_b200/csrc/plan.h"
 #include "tma_emu.h"
 
 namespace b200
@@ -28,555 +27,320 @@ namespace b200
   int check_cuda(cudaError_t, const char *) { return 0; }
   void count_launch() { }
 
-  template <class P, int recon, bool dagger, bool xpay, OpType op> int run_config(const LaunchRequest &rq, const DslashArgs<P, recon> &arg)
-  {
-    const Geom &g = arg.geom;
-    TileMap tm;
-    int threads, gx, gy, gz, rc;
-    if (int e = make_tile_map(tm, threads, rq.tile, g, 128)) return e;
-    const bool partitioned = arg.threads_ext[4] > 0;
-    long visited = 0;
-    // kernels.cuh::wait_for_halo: every role that reads ghost zones first acquires the arrival counters.  The twin runs
-    // pack and Dslash one after the other, so a counter below its target is a deadlock (or a 10 s timeout) on the GPU.
-    if (partitioned && rq.kernel != B200_KERNEL_INTERIOR && rq.kernel != B200_KERNEL_INTERIOR_TILES && rq.kernel != B200_KERNEL_INTERIOR_SITES) {
-      const unsigned uses = (arg.seq + (arg.seq & 1u)) >> 1;
-      for (int d = 0; d < 4; d++)
-        for (int dir = 0; dir < 2; dir++)
-          if (const unsigned *f = arg.wait_flag[d][dir]) {
-            const unsigned target = uses * (unsigned)g.face_cb[d];
-            if ((int)(*f - target) < 0)
-              return set_error(B200_ERR_INVALID, "halo wait would never finish: counter[%d][%d] = %u < %u (exchange %u)", d, dir, *f, target, arg.seq);
-          }
-    }
-    if (rq.tma && !partitioned && rq.kernel == B200_KERNEL_AUTO) { // capi.cu: TMA-staged marching kernel where it serves the shape
-      const int rc = tma_emu_launch<P, recon, dagger, xpay, op>(rq, arg);
-      if (rc != kTmaSkip) return rc;
-      if (rq.tma > 1) return set_error(B200_ERR_UNSUPPORTED, "B200_TMA=2: shape not served by the TMA kernel");
-    }
-    // walk the SAME launch grids as kernels.cuh::launch_config (tile boxes, slab table, block / thread decomposition)
-    auto walk_box = [&](auto site_fn) {
-#pragma omp parallel for collapse(2) reduction(+ : visited)
-      for (int bz = 0; bz < gz; bz++)
-        for (int by = 0; by < gy; by++)
-          for (int bx = 0; bx < gx; bx++)
-            for (int tid = 0; tid < threads; tid++) {
-              int x[4], x_cb, par;
-              if (!tile_site(x, x_cb, par, g, tm, arg.n_parity, arg.parity, bx, by, bz, tid)) continue;
-              site_fn(x, x_cb, par);
-              visited++;
-            }
-    };
-    const bool tiles_path
-      = rq.kernel == B200_KERNEL_AUTO || rq.kernel == B200_KERNEL_INTERIOR_TILES || rq.kernel == B200_KERNEL_BOUNDARY_TILES;
-    if (partitioned && arg.n_parity == 1 && (rq.kernel == B200_KERNEL_INTERIOR_SITES || rq.kernel == B200_KERNEL_BOUNDARY_SITES)) {
-      // the interior / boundary role of dslash_fused_kernel alone
-      if (rq.kernel == B200_KERNEL_INTERIOR_SITES) {
-        if (!box_grid(tm, arg.n_parity, gx, gy, gz, rc)) return rc ? rc : -1;
-        walk_box([&](const int *x, int x_cb, int par) {
-          if (site_is_interior(arg, x)) dslash_site_interior<P, recon, dagger, xpay, op, false>(arg, x, x_cb, par);
-        });
-      } else {
-        for (int tid = 0; tid < arg.threads_ext[4]; tid++) {
-          int x[4], x_cb;
-          if (exterior_thread_site(x, x_cb, arg, tid, arg.parity)) dslash_site_full<P, recon, dagger, xpay, op>(arg, x, x_cb, arg.parity);
-        }
-      }
-      return 0;
-    }
-    if (partitioned && rq.fused_pack && rq.kernel == B200_KERNEL_AUTO && arg.n_parity == 1) {
-      // kernels.cuh::dslash_fused_kernel: (the pack role ran in twin_dslash_apply_fused) interior role over every tile with
-      // the face sites retiring, boundary role over the face-site enumeration
-      if (!box_grid(tm, arg.n_parity, gx, gy, gz, rc)) return rc ? rc : -1;
-      walk_box([&](const int *x, int x_cb, int par) {
-        if (site_is_interior(arg, x)) dslash_site_interior<P, recon, dagger, xpay, op, false>(arg, x, x_cb, par);
-      });
-      long done = 0;
-      std::vector<char> seen(g.volume_cb, 0);
-      for (int tid = 0; tid < arg.threads_ext[4]; tid++) {
-        int x[4], x_cb;
-        if (!exterior_thread_site(x, x_cb, arg, tid, arg.parity)) continue;
-        if (seen[x_cb]++) return set_error(B200_ERR_INVALID, "fused boundary role visits site %d twice", x_cb);
-        if (site_is_interior(arg, x)) return set_error(B200_ERR_INVALID, "fused boundary role visits interior site %d", x_cb);
-        dslash_site_full<P, recon, dagger, xpay, op>(arg, x, x_cb, arg.parity);
-        done++;
-      }
-      // every face site exactly once: interior + boundary = all sites
-      long interior = 0;
-      for (int x_cb = 0; x_cb < g.volume_cb; x_cb++) {
-        int x[4];
-        coords_from_cb(x, g, x_cb, arg.parity);
-        if (site_is_interior(arg, x)) interior++;
-      }
-      if (interior + done != (long)g.volume_cb)
-        return set_error(B200_ERR_INVALID, "fused roles cover %ld interior + %ld boundary of %d sites", interior, done, g.volume_cb);
-      return 0;
-    }
-    if (tiles_path && partitioned) {
-      SlabTable st;
-      const int nb = split_boundary(tm, st, arg.comm_dim);
-      if (rq.kernel != B200_KERNEL_BOUNDARY_TILES) {
-        if (box_grid(tm, arg.n_parity, gx, gy, gz, rc))
-          walk_box([&](const int *x, int x_cb, int par) { dslash_site_interior<P, recon, dagger, xpay, op, false>(arg, x, x_cb, par); });
-        else if (rc)
-          return rc;
-      }
-      if (rq.kernel != B200_KERNEL_INTERIOR_TILES)
-      for (int pp = 0; pp < arg.n_parity; pp++) {
-        const int parity = arg.n_parity == 2 ? pp : arg.parity;
-#pragma omp parallel for reduction(+ : visited)
-        for (int bx = 0; bx < nb; bx++)
-          for (int tid = 0; tid < threads; tid++) {
-            int x[4], x_cb;
-            if (!slab_site(x, x_cb, g, tm, st, parity, bx, tid)) continue;
-            dslash_site_full<P, recon, dagger, xpay, op>(arg, x, x_cb, parity);
-            visited++;
-          }
-      }
-      if (rq.kernel == B200_KERNEL_AUTO && visited != (long)g.volume_cb * arg.n_parity)
-        return set_error(B200_ERR_INVALID, "interior box + boundary slabs visited %ld of %ld sites", visited,
-                         (long)g.volume_cb * arg.n_parity);
-      return 0;
-    }
-    if (rq.kernel != B200_KERNEL_EXTERIOR) {
-      if (!box_grid(tm, arg.n_parity, gx, gy, gz, rc)) return rc ? rc : -1;
-      if (partitioned)
-        walk_box([&](const int *x, int x_cb, int par) { dslash_site_interior<P, recon, dagger, xpay, op, true>(arg, x, x_cb, par); });
-      else
-        walk_box([&](const int *x, int x_cb, int par) { dslash_site_interior<P, recon, dagger, xpay, op, false>(arg, x, x_cb, par); });
-      if (visited != (long)g.volume_cb * arg.n_parity)
-        return set_error(B200_ERR_INVALID, "tile map visited %ld of %ld sites", visited, (long)g.volume_cb * arg.n_parity);
-    }
-    if (rq.kernel == B200_KERNEL_EXTERIOR) {
-      for (int pp = 0; pp < arg.n_parity; pp++) {
-        const int parity = arg.n_parity == 2 ? pp : arg.parity;
-#pragma omp parallel for
-        for (int tid = 0; tid < arg.threads_ext[4]; tid++) {
-          int x[4], x_cb;
-          if (exterior_thread_site(x, x_cb, arg, tid, parity)) dslash_site_exterior<P, recon, dagger, xpay, op>(arg, x, x_cb, parity);
-        }
-      }
-    }
-    return 0;
-  }
+  constexpr int kH100Sms = 132; // CTAs of the TMA kernel's persistent grid on an H100 (one per SM)
 
-  template <class P, int recon> int run_recon(const LaunchRequest &rq)
+  // kernels.cuh::wait_for_halo: every role that reads ghost zones first acquires the arrival counters.  The twin runs
+  // pack and Dslash one after the other, so a counter below its target is a deadlock (or a 10 s timeout) on the GPU.
+  template <class Arg> int check_halo_arrived(const Arg &arg)
   {
-    DslashArgs<P, recon> arg;
-    if (int rc = fill_args(arg, rq)) return rc;
-    const bool xp = rq.xpay, dg = rq.dagger;
-#define GO(D, X, O) return run_config<P, recon, D, X, O>(rq, arg)
-    switch (rq.op) {
-    case OP_WILSON:
-      if (dg) { if (xp) GO(true, true, OP_WILSON); else GO(true, false, OP_WILSON); }
-      else { if (xp) GO(false, true, OP_WILSON); else GO(false, false, OP_WILSON); }
-    case OP_CLOVER:
-      if (!xp) return set_error(B200_ERR_INVALID, "ApplyWilsonClover exists in xpay form only (a != 0)");
-      if (dg) GO(true, true, OP_CLOVER); else GO(false, true, OP_CLOVER);
-    case OP_CLOVER_PC:
-      if (dg) { if (xp) GO(true, true, OP_CLOVER_PC); else GO(true, false, OP_CLOVER_PC); }
-      else { if (xp) GO(false, true, OP_CLOVER_PC); else GO(false, false, OP_CLOVER_PC); }
-    case OP_TM:
-      if (dg) GO(true, true, OP_TM); else GO(false, true, OP_TM);
-    case OP_TM_PC:
-      if (dg && !rq.asymmetric) { if (xp) GO(true, true, OP_TM_PC_PRE); else GO(true, false, OP_TM_PC_PRE); }
-      if (dg) GO(true, false, OP_TM_PC);
-      if (xp) GO(false, true, OP_TM_PC); else GO(false, false, OP_TM_PC);
-    }
-#undef GO
-    return set_error(B200_ERR_INVALID, "unknown op");
-  }
-
-  template <class P> int run_precision(const LaunchRequest &rq)
-  {
-    switch (rq.reconstruct) {
-    case 18: return run_recon<P, 18>(rq);
-    case 12: return run_recon<P, 12>(rq);
-    case 8: return run_recon<P, 8>(rq);
-    }
-    return set_error(B200_ERR_INVALID, "reconstruct %d", rq.reconstruct);
-  }
-
-  // ---- multi-RHS: same batches (launch.h::mrhs_batch) and the same tile grid as mrhs.cuh
-  template <class P, int recon, bool dagger, bool xpay, OpType op, int NS>
-  int run_mrhs_batch(const MrhsRequest &rq, const DslashArgs<P, recon> &arg, int s0)
-  {
-    MrhsFields<P, NS> f;
-    fill_mrhs_fields(f, rq, s0);
-    const Geom &g = arg.geom;
-    TileMap tm;
-    int threads, gx, gy, gz, rc;
-    if (int e = make_tile_map(tm, threads, rq.base.tile, g, 128)) return e;
-    if (!mrhs_box(tm, rq, arg.comm_dim, arg.n_parity, gx, gy, gz, rc)) return rc;
-    long visited = 0;
-#pragma omp parallel for collapse(2) reduction(+ : visited)
-    for (int bz = 0; bz < gz; bz++)
-      for (int by = 0; by < gy; by++)
-        for (int bx = 0; bx < gx; bx++)
-          for (int tid = 0; tid < threads; tid++) {
-            int x[4], x_cb, par;
-            if (!tile_site(x, x_cb, par, g, tm, arg.n_parity, arg.parity, bx, by, bz, tid)) continue;
-            dslash_site_mrhs<P, recon, dagger, xpay, op, NS>(arg, f, x, x_cb, par);
-            visited++;
-          }
-    if (!rq.interior_box && visited != (long)g.volume_cb * arg.n_parity) return set_error(B200_ERR_INVALID, "multi-RHS tile map visited %ld sites", visited);
-    return 0;
-  }
-
-  template <class P> int run_precision(const LaunchRequest &rq);
-
-  // CTA flavour: walk blockIdx.x = tile * n_batch + batch and threadIdx = (site in tile, source in CTA) as mrhs.cuh does
-  template <class P, int recon, bool dagger, bool xpay, OpType op> int run_mrhs_cta(const MrhsRequest &rq, const DslashArgs<P, recon> &arg)
-  {
-    MrhsViews<P> f;
-    fill_mrhs_views(f, rq);
-    const Geom &g = arg.geom;
-    TileMap tm;
-    int threads, gx, gy, gz, rc, nsb, n_batch;
-    if (int e = make_tile_map(tm, threads, rq.base.tile, g, 128)) return e;
-    if (!mrhs_box(tm, rq, arg.comm_dim, arg.n_parity, gx, gy, gz, rc)) return rc;
-    mrhs_cta_shape(nsb, n_batch, rq.n_src, threads, 128, rq.cta_sources);
-    long visited = 0;
-#pragma omp parallel for collapse(2) reduction(+ : visited)
-    for (int bz = 0; bz < gz; bz++)
-      for (int by = 0; by < gy; by++)
-        for (int bx = 0; bx < gx * n_batch; bx++)
-          for (int ty = 0; ty < nsb; ty++)
-            for (int tid = 0; tid < threads; tid++) {
-              const unsigned tile = (unsigned)bx / (unsigned)n_batch;
-              const int s = (bx - (int)tile * n_batch) * nsb + ty;
-              if (s >= rq.n_src) continue;
-              int x[4], x_cb, par;
-              if (!tile_site(x, x_cb, par, g, tm, arg.n_parity, arg.parity, tile, by, bz, tid)) continue;
-              dslash_site_src<P, recon, dagger, xpay, op, Cache::REUSE>(arg, f.in[s][1 - par], f.out[s][par], f.x[s][par], x, x_cb, par);
-              visited++;
-            }
-    if (!rq.interior_box && visited != (long)g.volume_cb * arg.n_parity * rq.n_src)
-      return set_error(B200_ERR_INVALID, "multi-RHS (CTA) grid visited %ld (site, source) pairs", visited);
-    return 0;
-  }
-
-  template <class P, int recon, bool dagger, bool xpay, OpType op> int run_mrhs_config(const MrhsRequest &rq, const DslashArgs<P, recon> &arg)
-  {
-    if (mrhs_mode(rq, P::bytes) == 1) return run_mrhs_cta<P, recon, dagger, xpay, op>(rq, arg);
-    int s0 = 0;
-    while (s0 < rq.n_src) {
-      const int ns = mrhs_batch<P>(rq.n_src - s0, rq.max_batch);
-      int rc = 0;
-      if (ns == 4) {
-        rc = run_mrhs_batch<P, recon, dagger, xpay, op, 4>(rq, arg, s0);
-      } else if (ns == 2) {
-        rc = run_mrhs_batch<P, recon, dagger, xpay, op, 2>(rq, arg, s0);
-      } else {
-        LaunchRequest one = rq.base;
-        one.out = rq.out[s0];
-        one.in = rq.in[s0];
-        if (rq.base.xpay) one.x = rq.x[s0];
-        rc = run_precision<P>(one);
-      }
-      if (rc) return rc;
-      s0 += ns;
-    }
-    return 0;
-  }
-
-  template <class P, int recon> int run_mrhs_recon(const MrhsRequest &rq)
-  {
-    DslashArgs<P, recon> arg;
-    if (int rc = fill_args(arg, rq.base)) return rc;
-    const bool xp = rq.base.xpay, dg = rq.base.dagger;
-#define GO(D, X, O) return run_mrhs_config<P, recon, D, X, O>(rq, arg)
-    switch (rq.base.op) {
-    case OP_WILSON:
-      if (dg) { if (xp) GO(true, true, OP_WILSON); else GO(true, false, OP_WILSON); }
-      else { if (xp) GO(false, true, OP_WILSON); else GO(false, false, OP_WILSON); }
-    case OP_CLOVER:
-      if (!xp) return set_error(B200_ERR_INVALID, "ApplyWilsonClover exists in xpay form only (a != 0)");
-      if (dg) GO(true, true, OP_CLOVER); else GO(false, true, OP_CLOVER);
-    case OP_CLOVER_PC:
-      if (dg) { if (xp) GO(true, true, OP_CLOVER_PC); else GO(true, false, OP_CLOVER_PC); }
-      else { if (xp) GO(false, true, OP_CLOVER_PC); else GO(false, false, OP_CLOVER_PC); }
-    }
-#undef GO
-    return set_error(B200_ERR_INVALID, "unknown op");
-  }
-
-  template <class P> int run_mrhs_precision(const MrhsRequest &rq)
-  {
-    switch (rq.base.reconstruct) {
-    case 18: return run_mrhs_recon<P, 18>(rq);
-    case 12: return run_mrhs_recon<P, 12>(rq);
-    case 8: return run_mrhs_recon<P, 8>(rq);
-    }
-    return set_error(B200_ERR_INVALID, "reconstruct %d", rq.base.reconstruct);
-  }
-
-  template <class P> int run_clover(const b200_spinor *out, const b200_spinor *in, const b200_clover *Ac, int inverse, int parity)
-  {
-    SpinorView<P> o, i;
-    CloverView<P> A;
-    fill_spinor(o, out->v, out->norm, out->volume_cb);
-    fill_spinor(i, in->v, in->norm, in->volume_cb);
-    fill_clover(A, *Ac, out->volume_cb);
-    for (int x_cb = 0; x_cb < out->volume_cb; x_cb++) {
-      typename P::real v[24];
-      i.load(v, x_cb);
-      if (inverse)
-        clover_apply_site<P, true>(v, A, x_cb, parity);
-      else
-        clover_apply_site<P, false>(v, A, x_cb, parity);
-      o.save(v, x_cb);
-    }
-    return 0;
-  }
-
-  // same body as kernels.cuh::pack_site (which is __device__-only because of its blockIdx plumbing)
-  template <class P> int run_pack(const b200_pack_args *a)
-  {
-    Geom g;
-    geom_init(g, a->X);
-    SpinorView<P> in;
-    fill_spinor(in, a->in.v, a->in.norm, g.volume_cb);
-    for (int d = 0; d < 4; d++) {
-      if (!a->comm_dim[d]) continue;
-      for (int face = 0; face < 2; face++) {
-        GhostView<P> dst;
-        fill_ghost(dst, a->dst[d][face], a->dst_norm[d][face], g.face_cb[d]);
-        for (int idx = 0; idx < g.face_cb[d]; idx++) {
-          int x[4];
-          coords_from_face(x, g, d, face ? g.X[d] - 1 : 0, idx, a->parity);
-          const int x_cb = cb_from_coords(x, g);
-          const int sign = (face == 0) ? (a->dagger ? +1 : -1) : (a->dagger ? -1 : +1);
-          typename P::real v[24], h[12];
-          in.load(v, x_cb);
-          project(h, v, d, sign);
-          dst.save(h, idx);
-        }
-      }
-    }
-    return 0;
-  }
-
-  // kernels.cuh::pack_multi_kernel, CTA by CTA: grid (blocks over the largest face, 8 faces, n_src sources) walked in a
-  // scrambled order (CTAs retire in any order on the GPU), each CTA = 128 threads of pack_block with the source's views
-  // (launch.h::ghost_of_source, the function the kernel uses) followed by the ticket protocol: the CTA that draws ticket
-  // nblk * n_src - 1 of its face publishes the arrival count.  Checks on the way that the count is published exactly once
-  // per face and only after every site of every source has been written.
-  template <class P> int run_pack_multi(const b200_pack_args *a, int n_src, const b200_spinor *src, const size_t *dst_stride)
-  {
-    Geom g;
-    geom_init(g, a->X);
-    int max_face = 0;
+    const unsigned uses = (arg.seq + (arg.seq & 1u)) >> 1;
     for (int d = 0; d < 4; d++)
-      if (a->comm_dim[d] && g.face_cb[d] > max_face) max_face = g.face_cb[d];
-    if (max_face == 0) return 0;
-    const int block = 128, gx = (max_face + block - 1) / block;
+      for (int dir = 0; dir < 2; dir++)
+        if (const unsigned *f = arg.wait_flag[d][dir]) {
+          const unsigned target = uses * (unsigned)arg.geom.face_cb[d];
+          if ((int)(*f - target) < 0)
+            return set_error(B200_ERR_INVALID, "halo wait would never finish: counter[%d][%d] = %u < %u (exchange %u)", d, dir, *f, target, arg.seq);
+        }
+    return 0;
+  }
+
+  // A pack grid CTA by CTA in a scrambled order (CTAs retire in any order on the GPU).  cta(c, face_id, blk, nblk, views)
+  // describes CTA c (false: it has no work): its `block` threads run pack_site, then the ticket protocol of
+  // kernels.cuh::pack_block follows -- the CTA that draws ticket nblk - 1 of its face publishes the arrival count.  Checks
+  // on the way that the count is published exactly once per face and only after every site of all `n_src` sources landed.
+  template <class P, class Cta> int walk_pack(const PackArgs<P> &arg, long n_cta, int block, int n_src, Cta &&cta)
+  {
+    const Geom &g = arg.geom;
     int tickets[8] = {0}, published[8] = {0};
     long written[8] = {0};
-    const long n_cta = (long)gx * 8 * n_src;
     // an odd multiplier coprime to n_cta visits every CTA exactly once in a scrambled order
     long mul = 7919;
     while (std::gcd(mul, n_cta) != 1) mul += 2;
     for (long k = 0; k < n_cta; k++) {
-      const long c = (k * mul + 12345) % n_cta;
-      const int bx = (int)(c % gx), by = (int)((c / gx) % 8), s = (int)(c / ((long)gx * 8));
-      const int d = by >> 1, face = by & 1;
-      if (!a->comm_dim[d]) continue;
-      const int nblk = (g.face_cb[d] + block - 1) / block;
-      if (bx >= nblk) continue;
-      SpinorView<P> in;
-      fill_spinor(in, src[s].v, src[s].norm, g.volume_cb);
-      GhostView<P> first;
-      fill_ghost(first, a->dst[d][face], a->dst_norm[d][face], g.face_cb[d]);
-      const GhostView<P> dst = ghost_of_source(first, (size_t)s * dst_stride[d]);
+      int f, blk, nblk;
+      PackSourceViews<P> vw;
+      if (!cta((k * mul + 12345) % n_cta, f, blk, nblk, vw)) continue;
+      const int d = f >> 1, face = f & 1;
       for (int tid = 0; tid < block; tid++) {
-        const int idx = bx * block + tid;
+        const int idx = blk * block + tid;
         if (idx >= g.face_cb[d]) continue;
-        int x[4];
-        coords_from_face(x, g, d, face ? g.X[d] - 1 : 0, idx, a->parity);
-        const int x_cb = cb_from_coords(x, g);
-        const int sign = (face == 0) ? (a->dagger ? +1 : -1) : (a->dagger ? -1 : +1);
-        typename P::real v[24], h[12];
-        in.load(v, x_cb);
-        project(h, v, d, sign);
-        dst.save(h, idx);
-        written[by]++;
+        pack_site(arg, vw, d, face, idx);
+        written[f]++;
       }
-      if (a->signal[d][face]) {
-        if (!a->block_counter) return set_error(B200_ERR_INVALID, "signal[] given without block_counter scratch");
-        const int prev = tickets[by]++;
-        if (prev == nblk * n_src - 1) {
-          if (written[by] != (long)n_src * g.face_cb[d]) return set_error(B200_ERR_INVALID, "face %d signalled before all sources landed", by);
-          if (published[by]++) return set_error(B200_ERR_INVALID, "face %d signalled twice", by);
-          tickets[by] = 0;
-          const unsigned uses = (a->seq + (a->seq & 1u)) >> 1;
-          *static_cast<unsigned *>(a->signal[d][face]) = uses * (unsigned)g.face_cb[d];
+      if (unsigned *sig = arg.signal[d][face]) {
+        const int prev = tickets[f]++;
+        if (prev == nblk - 1) {
+          if (written[f] != (long)n_src * g.face_cb[d]) return set_error(B200_ERR_INVALID, "face %d signalled before all sources landed", f);
+          if (published[f]++) return set_error(B200_ERR_INVALID, "face %d signalled twice", f);
+          tickets[f] = 0;
+          *sig = ((arg.seq + (arg.seq & 1u)) >> 1) * (unsigned)g.face_cb[d];
         }
       }
     }
-    for (int by = 0; by < 8; by++)
-      if (a->comm_dim[by >> 1] && a->signal[by >> 1][by & 1] && published[by] != 1)
-        return set_error(B200_ERR_INVALID, "face %d never signalled", by);
+    for (int f = 0; f < 8; f++)
+      if (arg.signal[f >> 1][f & 1] && published[f] != 1) return set_error(B200_ERR_INVALID, "face %d never signalled", f);
     return 0;
   }
+
+  // one planned Dslash (plan.h::plan_dslash), launch by launch as kernels.cuh::launch_config issues it.  Counts the site
+  // updates on the way: no launch plan may update a site twice, and a plan for the whole operator updates every one.
+  template <class P, int recon, bool dagger, bool xpay, OpType op>
+  int run_config(OpCfg<dagger, xpay, op>, const LaunchRequest &rq, const DslashArgs<P, recon> &arg)
+  {
+    LaunchPlan pl;
+    if (int rc = plan_dslash(pl, rq, arg)) return rc;
+    const Geom &g = arg.geom;
+    std::vector<int> hits(2 * (size_t)g.volume_cb, 0);
+    auto twice = [&](int par, int x_cb) -> long {
+      int prev;
+#pragma omp atomic capture
+      prev = hits[(size_t)par * g.volume_cb + x_cb]++;
+      return prev != 0;
+    };
+    long repeats = 0;
+    for (int i = 0; i < pl.n; i++) {
+      const LaunchStep &l = pl.step[i];
+      const TileMap &tm = l.tm;
+      if (l.kind == LAUNCH_INTERIOR) {
+#pragma omp parallel for collapse(2) reduction(+ : repeats)
+        for (int bz = 0; bz < l.grid[2]; bz++)
+          for (int by = 0; by < l.grid[1]; by++)
+            for (int bx = 0; bx < l.grid[0]; bx++)
+              for (int tid = 0; tid < l.threads; tid++) {
+                int x[4], x_cb, par;
+                if (!tile_site(x, x_cb, par, g, tm, arg.n_parity, arg.parity, bx, by, bz, tid)) continue;
+                if (l.masked)
+                  dslash_site_interior<P, recon, dagger, xpay, op, true>(arg, x, x_cb, par);
+                else
+                  dslash_site_interior<P, recon, dagger, xpay, op, false>(arg, x, x_cb, par);
+                repeats += twice(par, x_cb);
+              }
+        continue;
+      }
+      if (l.kind == LAUNCH_FUSED) {
+        // dslash_fused_kernel: the pack CTAs first (all faces land before any boundary CTA waits), then blocks n_pack + b
+        const FusedShape &fs = l.fs;
+        if (fs.n_pack) {
+          PackArgs<P> pk;
+          fill_pack_args(pk, *rq.fused_pack);
+          const int rc = walk_pack(pk, fs.n_pack, l.threads, 1, [&](long c, int &f, int &blk, int &nblk, PackSourceViews<P> &vw) {
+            const int b = (int)c;
+            f = fused_pack_face(fs, b);
+            blk = b - fs.pack_start[f];
+            nblk = fs.pack_start[f + 1] - fs.pack_start[f];
+            vw = PackSourceViews<P> {pk.in, pk.dst[f >> 1][f & 1]};
+            return true;
+          });
+          if (rc) return rc;
+        }
+        if (fs.n_boundary)
+          if (int rc = check_halo_arrived(arg)) return rc;
+#pragma omp parallel for reduction(+ : repeats)
+        for (int b = 0; b < l.grid[0] - fs.n_pack; b++) {
+          const int ib = fused_interior_tile(fs, b);
+          int bx = 0, by = 0, bz = 0;
+          if (ib >= 0) fused_tile_block(fs, ib, bx, by, bz);
+          for (int tid = 0; tid < l.threads; tid++) {
+            int x[4], x_cb, par = arg.parity;
+            if (ib >= 0) {
+              if (!tile_site(x, x_cb, par, g, tm, arg.n_parity, arg.parity, bx, by, bz, tid) || !site_is_interior(arg, x)) continue;
+              dslash_site_interior<P, recon, dagger, xpay, op, false>(arg, x, x_cb, par);
+            } else {
+              const int t = (b - fs.n_interior_first) * l.threads + tid;
+              if (t >= arg.threads_ext[4] || !exterior_thread_site(x, x_cb, arg, t, par)) continue;
+              dslash_site_full<P, recon, dagger, xpay, op>(arg, x, x_cb, par);
+            }
+            repeats += twice(par, x_cb);
+          }
+        }
+        continue;
+      }
+      if (int rc = check_halo_arrived(arg)) return rc;
+      for (int by = 0; by < l.grid[1]; by++) {
+        const int par = arg.n_parity == 2 ? by : arg.parity;
+#pragma omp parallel for reduction(+ : repeats)
+        for (int bx = 0; bx < l.grid[0]; bx++)
+          for (int tid = 0; tid < l.threads; tid++) {
+            int x[4], x_cb;
+            if (l.kind == LAUNCH_BOUNDARY) {
+              if (!slab_site(x, x_cb, g, tm, l.st, par, bx, tid)) continue;
+              dslash_site_full<P, recon, dagger, xpay, op>(arg, x, x_cb, par);
+            } else {
+              const int t = bx * l.threads + tid;
+              if (t >= arg.threads_ext[4] || !exterior_thread_site(x, x_cb, arg, t, par)) continue;
+              dslash_site_exterior<P, recon, dagger, xpay, op>(arg, x, x_cb, par);
+            }
+            repeats += twice(par, x_cb);
+          }
+      }
+    }
+    if (repeats) return set_error(B200_ERR_INVALID, "the launch plan updates %ld sites more than once", repeats);
+    const long updated = std::accumulate(hits.begin(), hits.end(), 0L), all = (long)g.volume_cb * arg.n_parity;
+    if (pl.whole && updated != all) return set_error(B200_ERR_INVALID, "the launch plan updates %ld of %ld sites", updated, all);
+    return 0;
+  }
+
+  // one multi-RHS launch as mrhs.cuh issues it: the CTA flavour (NS == 0: blockIdx.x = tile * n_batch + batch, threadIdx =
+  // (site in tile, source in CTA)) or NS sources per thread from source s0 on
+  template <int NS, class P, int recon, bool dagger, bool xpay, OpType op>
+  int run_mrhs(OpCfg<dagger, xpay, op>, const MrhsRequest &rq, const DslashArgs<P, recon> &arg, int s0)
+  {
+    MrhsGrid m;
+    if (int rc = plan_mrhs(m, rq, arg, NS == 0)) return rc;
+    if (!m.gx) return 0;
+    MrhsViews<P> views;
+    MrhsFields<P, NS ? NS : 1> fields;
+    if constexpr (NS == 0)
+      fill_mrhs_views(views, rq);
+    else
+      fill_mrhs_fields(fields, rq, s0);
+    const Geom &g = arg.geom;
+    long visited = 0;
+#pragma omp parallel for collapse(2) reduction(+ : visited)
+    for (int bz = 0; bz < m.gz; bz++)
+      for (int by = 0; by < m.gy; by++)
+        for (int bx = 0; bx < m.gx * m.n_batch; bx++)
+          for (int ty = 0; ty < m.nsb; ty++)
+            for (int tid = 0; tid < m.threads; tid++) {
+              const unsigned tile = (unsigned)bx / (unsigned)m.n_batch;
+              const int s = (bx - (int)tile * m.n_batch) * m.nsb + ty;
+              if (s >= rq.n_src) continue;
+              int x[4], x_cb, par;
+              if (!tile_site(x, x_cb, par, g, m.tm, arg.n_parity, arg.parity, tile, by, bz, tid)) continue;
+              if constexpr (NS == 0)
+                dslash_site_src<P, recon, dagger, xpay, op, Cache::REUSE>(arg, views.in[s][1 - par], views.out[s][par], views.x[s][par], x, x_cb, par);
+              else
+                dslash_site_mrhs<P, recon, dagger, xpay, op, NS>(arg, fields, x, x_cb, par);
+              visited++;
+            }
+    const long want = (long)g.volume_cb * arg.n_parity * (NS == 0 ? rq.n_src : 1);
+    if (!rq.interior_box && visited != want) return set_error(B200_ERR_INVALID, "multi-RHS grid visited %ld of %ld (site, source) pairs", visited, want);
+    return 0;
+  }
+
+  // the executor of plan.h's entry points: CPU walkers of the launch grids the CUDA launchers issue
+  struct Twin {
+    static int require_device() { return 0; }
+
+    template <class P> static int dslash(const LaunchRequest &rq)
+    {
+      return dispatch_dslash<P>(rq, [&](auto c, const auto &arg) { return run_config(c, rq, arg); });
+    }
+
+    template <class P> static int tma(const LaunchRequest &rq)
+    {
+      return dispatch_tma<P>(rq, [&](auto c, const auto &arg) { return tma_emu_launch(c, rq, arg, kH100Sms); });
+    }
+
+    template <class P> static int mrhs(const MrhsRequest &rq)
+    {
+      return dispatch_mrhs<P>(rq, [&](auto c, const auto &arg, auto ns, int s0) -> int {
+        constexpr int NS = decltype(ns)::value;
+        if constexpr (NS == 1)
+          return dslash<P>(mrhs_source(rq, s0));
+        else
+          return run_mrhs<NS>(c, rq, arg, s0);
+      });
+    }
+
+    // clover_apply_kernel / twist_gamma5_kernel: one thread per site
+    template <class P> static int clover(const CloverRequest &rq)
+    {
+      SpinorView<P> out, in;
+      CloverView<P> A;
+      fill_spinor(out, rq.out, rq.out_norm, rq.volume_cb);
+      fill_spinor(in, rq.in, rq.in_norm, rq.volume_cb);
+      fill_clover(A, rq.A, rq.volume_cb);
+      for (int x_cb = 0; x_cb < rq.volume_cb; x_cb++) {
+        typename P::real v[24];
+        in.load(v, x_cb);
+        if (rq.inverse)
+          clover_apply_site<P, true>(v, A, x_cb, rq.parity);
+        else
+          clover_apply_site<P, false>(v, A, x_cb, rq.parity);
+        out.save(v, x_cb);
+      }
+      return 0;
+    }
+
+    template <class P> static int twist(const TwistRequest &rq)
+    {
+      SpinorView<P> out, in;
+      fill_spinor(out, rq.out, rq.out_norm, rq.volume_cb);
+      fill_spinor(in, rq.in, rq.in_norm, rq.volume_cb);
+      for (int x_cb = 0; x_cb < rq.volume_cb; x_cb++) {
+        typename P::real v[24];
+        in.load(v, x_cb);
+        twist_apply(v, (typename P::real)rq.a, (typename P::real)rq.b);
+        out.save(v, x_cb);
+      }
+      return 0;
+    }
+
+    // pack_multi_kernel: grid (blocks over the largest face, 8 face ids, n_src sources) of 128 threads
+    template <class P> static int pack_multi(const PackRequest &rq, const PackBatchRequest &b)
+    {
+      int gx;
+      if (int rc = pack_blocks(gx, rq)) return rc;
+      if (!gx) return 0;
+      PackArgs<P> arg;
+      fill_pack_args(arg, rq);
+      PackBatch<P> batch;
+      fill_pack_batch(batch, b, arg.geom.volume_cb);
+      return walk_pack(arg, (long)gx * 8 * b.n_src, 128, b.n_src, [&](long c, int &f, int &blk, int &nblk, PackSourceViews<P> &vw) {
+        blk = (int)(c % gx);
+        f = (int)((c / gx) % 8);
+        const int s = (int)(c / ((long)gx * 8)), d = f >> 1;
+        const int n = (arg.geom.face_cb[d] + 127) / 128;
+        if (!arg.comm_dim[d] || blk >= n) return false;
+        nblk = n * batch.n_src;
+        vw = PackSourceViews<P> {arg.in, ghost_of_source(arg.dst[d][f & 1], (size_t)s * batch.dst_stride[d])};
+        vw.in_.v = batch.in[s];
+        vw.in_.norm = batch.in_norm[s];
+        return true;
+      });
+    }
+
+    // pack_kernel: the same grid with one source, its own field
+    template <class P> static int pack(const PackRequest &rq)
+    {
+      PackBatchRequest one {};
+      one.n_src = 1;
+      one.in[0] = rq.in;
+      one.in_norm[0] = rq.in_norm;
+      return pack_multi<P>(rq, one);
+    }
+  };
 } // namespace b200
 
 using namespace b200;
 
-template <class P> static int run_twist(const b200_spinor *out, const b200_spinor *in, double a, double b)
-{
-  SpinorView<P> o, i;
-  fill_spinor(o, out->v, out->norm, out->volume_cb);
-  fill_spinor(i, in->v, in->norm, in->volume_cb);
-  for (int x_cb = 0; x_cb < out->volume_cb; x_cb++) {
-    typename P::real v[24];
-    i.load(v, x_cb);
-    twist_apply(v, (typename P::real)a, (typename P::real)b);
-    o.save(v, x_cb);
-  }
-  return 0;
-}
-
 extern "C" {
 const char *twin_last_error(void) { return g_err; }
 
-int twin_dslash_apply(const b200_dslash_args *a)
-{
-  LaunchRequest rq;
-  bool nothing = false;
-  if (int rc = make_request(rq, a, nothing)) return rc;
-  if (nothing) return 0;
-  if (const char *e = getenv("B200_TMA")) rq.tma = atoi(e); // (read on every call: tests toggle it)
-  if (const char *e = getenv("B200_TMA_TILE")) sscanf(e, "%d %d", &rq.tma_ty, &rq.tma_tz);
-  if (const char *e = getenv("B200_TMA_GRID")) rq.tma_grid = atoi(e);
-  if (const char *e = getenv("B200_TMA_LINKS")) rq.tma_link_slots = atoi(e);
-  if (const char *e = getenv("B200_TMA_PREFETCH")) rq.tma_prefetch = atoi(e);
-  if (const char *e = getenv("B200_TMA_L2PF")) rq.tma_l2_prefetch = atoi(e);
-  if (const char *e = getenv("B200_TMA_RINGS")) sscanf(e, "%d %d", &rq.tma_center_slots, &rq.tma_halo_slots);
-  switch (a->precision) {
-  case B200_DOUBLE: return run_precision<PrecF64>(rq);
-  case B200_SINGLE: return run_precision<PrecF32>(rq);
-  case B200_HALF: return run_precision<PrecH16>(rq);
-  }
-  return -1;
-}
+int twin_dslash_apply(const b200_dslash_args *a) { return apply_dslash<Twin>(a); }
 
-int twin_pack_ghost(const b200_pack_args *a);
-
-int twin_dslash_apply_fused(const b200_dslash_args *a, const b200_pack_args *p)
-{
-  // same argument checks as capi.cu::b200_dslash_apply_fused
-  if (!a || !p) return set_error(B200_ERR_INVALID, "null argument");
-  if (a->kernel != B200_KERNEL_AUTO) return set_error(B200_ERR_INVALID, "the fused Dslash is the B200_KERNEL_AUTO schedule");
-  if (p->in.v != a->in.v || p->precision != a->precision || p->parity != 1 - a->parity || (p->dagger != 0) != (a->dagger != 0))
-    return set_error(B200_ERR_INVALID, "pack arguments do not describe the faces of this Dslash's input");
-  bool any = false;
-  for (int d = 0; d < 4; d++) {
-    if ((p->comm_dim[d] != 0) != (a->halo.comm_dim[d] != 0)) return set_error(B200_ERR_INVALID, "pack / halo partitioning differ");
-    any |= a->halo.comm_dim[d] != 0;
-  }
-  if (!any) return twin_dslash_apply(a);
-  if (int rc = twin_pack_ghost(p)) return rc; // the pack role (sequential emulation: all faces land before anybody waits)
-  LaunchRequest rq;
-  bool nothing = false;
-  if (int rc = make_request(rq, a, nothing)) return rc;
-  PackRequest marker {};
-  rq.fused_pack = &marker;
-  switch (a->precision) {
-  case B200_DOUBLE: return run_precision<PrecF64>(rq);
-  case B200_SINGLE: return run_precision<PrecF32>(rq);
-  case B200_HALF: return run_precision<PrecH16>(rq);
-  }
-  return -1;
-}
+int twin_dslash_apply_fused(const b200_dslash_args *a, const b200_pack_args *p) { return apply_dslash_fused<Twin>(a, p); }
 
 int twin_dslash_apply_multi(const b200_dslash_args *a, int n_src, const b200_spinor *out, const b200_spinor *in, const b200_spinor *x)
 {
-  MrhsRequest rq;
-  bool batched = false;
-  if (int rc = make_mrhs_request(rq, a, n_src, out, in, x, batched)) return rc;
-  if (!batched) {
-    for (int i = 0; i < n_src; i++) {
-      const b200_dslash_args one = source_args(*a, i, out, in, x);
-      if (int rc = twin_dslash_apply(&one)) return rc;
-    }
-    return 0;
-  }
-  if (rq.interior_box && a->kernel == B200_KERNEL_AUTO) { // capi.cu: batched interior, then every source's boundary tiles
-    b200_dslash_args interior = *a;
-    interior.kernel = B200_KERNEL_INTERIOR_TILES;
-    if (int rc = twin_dslash_apply_multi(&interior, n_src, out, in, x)) return rc;
-    for (int i = 0; i < n_src; i++) {
-      b200_dslash_args one = source_args(*a, i, out, in, x);
-      one.kernel = B200_KERNEL_BOUNDARY_TILES;
-      if (int rc = twin_dslash_apply(&one)) return rc;
-    }
-    return 0;
-  }
-  if (const char *e = getenv("B200_MRHS_MODE")) rq.mode = (strcmp(e, "cta") == 0) ? 1 : (strcmp(e, "thread") == 0 ? 0 : -1);
-  if (const char *e = getenv("B200_MRHS_BATCH")) rq.max_batch = atoi(e);
-  if (const char *e = getenv("B200_MRHS_CTA_SOURCES")) rq.cta_sources = atoi(e);
-  switch (a->precision) {
-  case B200_DOUBLE: return run_mrhs_precision<PrecF64>(rq);
-  case B200_SINGLE: return run_mrhs_precision<PrecF32>(rq);
-  case B200_HALF: return run_mrhs_precision<PrecH16>(rq);
-  }
-  return -1;
+  return apply_dslash_multi<Twin>(a, n_src, out, in, x);
 }
 
-int twin_clover_apply(const b200_spinor *out, const b200_spinor *in, const b200_clover *A, int precision, int inverse, int parity, void *)
+int twin_clover_apply(const b200_spinor *out, const b200_spinor *in, const b200_clover *A, int precision, int inverse, int parity, void *stream)
 {
-  switch (precision) {
-  case B200_DOUBLE: return run_clover<PrecF64>(out, in, A, inverse, parity);
-  case B200_SINGLE: return run_clover<PrecF32>(out, in, A, inverse, parity);
-  case B200_HALF: return run_clover<PrecH16>(out, in, A, inverse, parity);
-  }
-  return -1;
+  return clover_apply<Twin>(out, in, A, precision, inverse, parity, stream);
 }
 
-int twin_twist_gamma5(const b200_spinor *out, const b200_spinor *in, int precision, double kappa, double mu, int dagger, int inverse, void *)
+int twin_twist_gamma5(const b200_spinor *out, const b200_spinor *in, int precision, double kappa, double mu, int dagger, int inverse, void *stream)
 {
-  double a, b; // capi.cu::twist_coefficients
-  if (!inverse) { b = 2.0 * kappa * mu; a = 1.0; } else { b = -2.0 * kappa * mu; a = 1.0 / (1.0 + b * b); }
-  if (dagger) b = -b;
-  switch (precision) {
-  case B200_DOUBLE: return run_twist<PrecF64>(out, in, a, b);
-  case B200_SINGLE: return run_twist<PrecF32>(out, in, a, b);
-  case B200_HALF: return run_twist<PrecH16>(out, in, a, b);
-  }
-  return -1;
+  return twist_gamma5<Twin>(out, in, precision, kappa, mu, dagger, inverse, stream);
 }
 
 int twin_pack_ghost_multi(const b200_pack_args *a, int n_src, const b200_spinor *in, const size_t dst_stride[4])
 {
-  // same argument checks as capi.cu::b200_pack_ghost_multi
-  if (n_src < 1 || n_src > B200_MAX_MULTI_RHS) return set_error(B200_ERR_INVALID, "n_src %d not in [1, %d]", n_src, B200_MAX_MULTI_RHS);
-  if (!a || !in || !dst_stride) return set_error(B200_ERR_INVALID, "null argument");
-  for (int s = 0; s < n_src; s++) {
-    if (!in[s].v) return set_error(B200_ERR_INVALID, "source %d is null", s);
-    if (in[s].n_parity != 1) return set_error(B200_ERR_INVALID, "the batched pack takes single-parity sources");
-  }
-  for (int d = 0; d < 4; d++)
-    if (a->comm_dim[d] && !(a->dst[d][0] && a->dst[d][1])) return set_error(B200_ERR_INVALID, "dst[%d] is NULL", d);
-  if (int rc = check_src_stride("dst_stride", n_src, a->precision, a->X, a->comm_dim, dst_stride, 1)) return rc;
-  switch (a->precision) {
-  case B200_DOUBLE: return run_pack_multi<PrecF64>(a, n_src, in, dst_stride);
-  case B200_SINGLE: return run_pack_multi<PrecF32>(a, n_src, in, dst_stride);
-  case B200_HALF: return run_pack_multi<PrecH16>(a, n_src, in, dst_stride);
-  }
-  return -1;
+  return pack_ghost_multi<Twin>(a, n_src, in, dst_stride);
 }
 
-int twin_pack_ghost(const b200_pack_args *a)
-{
-  if (a->signal[0][0] || a->signal[1][0] || a->signal[2][0] || a->signal[3][0]) { // with arrival counters: the CTA walk
-    const size_t none[4] = {0, 0, 0, 0};
-    return twin_pack_ghost_multi(a, 1, &a->in, none);
-  }
-  switch (a->precision) {
-  case B200_DOUBLE: return run_pack<PrecF64>(a);
-  case B200_SINGLE: return run_pack<PrecF32>(a);
-  case B200_HALF: return run_pack<PrecH16>(a);
-  }
-  return -1;
-}
+int twin_pack_ghost(const b200_pack_args *a) { return pack_ghost<Twin>(a); }
 }

@@ -255,51 +255,46 @@ namespace b200
     return 0;
   }
 
-  // whole launch; kTmaSkip if the shape is not served (the caller then walks the gather kernel's grid)
+  // whole launch on a grid of (at most) n_sm CTAs; kTmaSkip if the shape is not served (the caller then walks the gather
+  // kernel's grid).  Which ops the kernel serves: plan.h::dispatch_tma.
   template <class P, int recon, bool dagger, bool xpay, OpType op>
-  int tma_emu_launch(const LaunchRequest &rq, const DslashArgs<P, recon> &arg)
+  int tma_emu_launch(OpCfg<dagger, xpay, op>, const LaunchRequest &rq, const DslashArgs<P, recon> &arg, int n_sm)
   {
-    if constexpr (P::fixed || op == OP_TM || op == OP_TM_PC || op == OP_TM_PC_PRE) {
-      return kTmaSkip;
-    } else {
-      if (op == OP_CLOVER_PC && dagger && xpay) return kTmaSkip;
-      TmaPlan plan;
-      TmaKnobs knobs {rq.tma_ty, rq.tma_tz, rq.tma_link_slots, rq.tma_center_slots, rq.tma_halo_slots, rq.tma_l2_prefetch};
-      if (!tma_make_plan<P, recon>(plan, arg.geom, arg.n_parity, arg.parity, knobs)) return kTmaSkip;
-      if (plan.smem_bytes > kTmaSmemBudget) return set_error(B200_ERR_INVALID, "TMA plan needs %d bytes of shared memory", plan.smem_bytes);
-      TmaDesc descs[2][TM_COUNT];
-      for (int pi = 0; pi < arg.n_parity; pi++) {
-        tma_make_descs(descs[pi], arg, plan, arg.n_parity == 2 ? pi : arg.parity);
-        for (int k = 0; k < TM_COUNT; k++)
-          if (!tma_desc_ok(descs[pi][k])) return kTmaSkip;
-      }
-      int grid = rq.tma_grid > 0 ? rq.tma_grid : 148;
-      if (grid > plan.n_items) grid = plan.n_items;
-      long visited = 0;
-      int err = 0;
-#pragma omp parallel for reduction(+ : visited) schedule(dynamic)
-      for (int cta = 0; cta < grid; cta++) {
-        long v = 0;
-        int e;
-        if (plan.n_link_slots > 0)
-          e = tma_emu_cta<P, recon, dagger, xpay, op, 0>(arg, plan, descs, cta, grid, v);
-        else if (rq.tma_prefetch == 2)
-          e = tma_emu_cta<P, recon, dagger, xpay, op, 2>(arg, plan, descs, cta, grid, v);
-        else if (rq.tma_prefetch == 4)
-          e = tma_emu_cta<P, recon, dagger, xpay, op, 4>(arg, plan, descs, cta, grid, v);
-        else
-          e = tma_emu_cta<P, recon, dagger, xpay, op, 3>(arg, plan, descs, cta, grid, v);
-        visited += v;
-        if (e) {
-#pragma omp critical
-          err = e;
-        }
-      }
-      if (err) return err;
-      if (visited != (long)arg.geom.volume_cb * arg.n_parity)
-        return set_error(B200_ERR_INVALID, "TMA work ranges visited %ld of %ld sites", visited, (long)arg.geom.volume_cb * arg.n_parity);
-      return 0;
+    TmaPlan plan;
+    TmaKnobs knobs {rq.tma_ty, rq.tma_tz, rq.tma_link_slots, rq.tma_center_slots, rq.tma_halo_slots, rq.tma_l2_prefetch};
+    if (!tma_make_plan<P, recon>(plan, arg.geom, arg.n_parity, arg.parity, knobs)) return kTmaSkip;
+    if (plan.smem_bytes > kTmaSmemBudget) return set_error(B200_ERR_INVALID, "TMA plan needs %d bytes of shared memory", plan.smem_bytes);
+    TmaDesc descs[2][TM_COUNT];
+    for (int pi = 0; pi < arg.n_parity; pi++) {
+      tma_make_descs(descs[pi], arg, plan, arg.n_parity == 2 ? pi : arg.parity);
+      for (int k = 0; k < TM_COUNT; k++)
+        if (!tma_desc_ok(descs[pi][k])) return kTmaSkip;
     }
+    const int grid = tma_grid(rq, plan.n_items, n_sm);
+    long visited = 0;
+    int err = 0;
+#pragma omp parallel for reduction(+ : visited) schedule(dynamic)
+    for (int cta = 0; cta < grid; cta++) {
+      long v = 0;
+      int e;
+      if (plan.n_link_slots > 0)
+        e = tma_emu_cta<P, recon, dagger, xpay, op, 0>(arg, plan, descs, cta, grid, v);
+      else if (rq.tma_prefetch == 2)
+        e = tma_emu_cta<P, recon, dagger, xpay, op, 2>(arg, plan, descs, cta, grid, v);
+      else if (rq.tma_prefetch == 4)
+        e = tma_emu_cta<P, recon, dagger, xpay, op, 4>(arg, plan, descs, cta, grid, v);
+      else
+        e = tma_emu_cta<P, recon, dagger, xpay, op, 3>(arg, plan, descs, cta, grid, v);
+      visited += v;
+      if (e) {
+#pragma omp critical
+        err = e;
+      }
+    }
+    if (err) return err;
+    if (visited != (long)arg.geom.volume_cb * arg.n_parity)
+      return set_error(B200_ERR_INVALID, "TMA work ranges visited %ld of %ld sites", visited, (long)arg.geom.volume_cb * arg.n_parity);
+    return 0;
   }
 
 } // namespace b200

@@ -222,9 +222,10 @@ def check_partitioned(mem, be, prec, recon, comm_dim, op="wilson", X=(4, 4, 4, 4
         halo = self_halo(P, mem, comm_dim)
         din = P.to_dev(s)
         fused_kw = {}
-        if split == "fused":  # pack + interior + boundary in one call (b200_dslash_apply_fused); host twin only: without
-            # arrival flags the real kernel's boundary CTAs would not wait for its pack CTAs
-            fused_kw = dict(fused_dst=[[halo.ghost[d][1], halo.ghost[d][0]] if comm_dim[d] else [None, None] for d in range(4)])
+        if split in ("fused", "fused_roles"):  # pack + interior + boundary in one call (b200_dslash_apply_fused); host twin
+            # only: without arrival flags the real kernel's boundary CTAs would not wait for its pack CTAs
+            fused_kw = dict(fused_dst=[[halo.ghost[d][1], halo.ghost[d][0]] if comm_dim[d] else [None, None] for d in range(4)],
+                            block_counter=mem.empty(32))
         else:
             self_exchange(P, halo, din, 1 - parity, dagger, be)
         out = P.empty()
@@ -234,6 +235,9 @@ def check_partitioned(mem, be, prec, recon, comm_dim, op="wilson", X=(4, 4, 4, 4
             kws = [dict(kernel=4, tile=tile), dict(kernel=3, tile=tile)]
         elif split == "sites":    # the same split with 1-site-thick shells (B200_KERNEL_BOUNDARY_SITES, then INTERIOR_SITES)
             kws = [dict(kernel=6, tile=tile), dict(kernel=5, tile=tile)]
+        elif split == "fused_roles":  # the fused launch's roles as the `split` halo schedule issues them: pack + boundary
+            # (B200_KERNEL_BOUNDARY_TILES), then the interior (B200_KERNEL_INTERIOR_TILES)
+            kws = [dict(kernel=4, tile=tile, **fused_kw), dict(kernel=3, tile=tile, **fused_kw)]
         elif split and split != "fused":  # reference-style: masked INTERIOR then EXTERIOR read-modify-write
             kws = [dict(kernel=1, tile=tile), dict(kernel=2, tile=tile)]
         else:

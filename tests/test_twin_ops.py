@@ -156,12 +156,14 @@ def test_twisted_mass_argument_checks():
         D.ApplyTwistedMassPreconditioned(out, s, P.U, 1.0, 0.1, False, None, 0, 1, False, halo=h, backend=be)
 
 
+@pytest.mark.parametrize("split", ["fused", "fused_roles"])
 @pytest.mark.parametrize("comm_dim", MASKS)
-def test_fused_single_launch_all_masks(comm_dim):
-    """b200_dslash_apply_fused (pack + interior + boundary as one launch): the interior role (every tile, face sites
-    retire) and the boundary role (one thread per face site, corners owned by the highest partitioned dimension) must
-    cover every site exactly once and reproduce the periodic operator for all 15 partition masks"""
-    ops.check_partitioned(HostMem, twin_backend(), 8, 18, comm_dim, X=(4, 6, 4, 8), split="fused")
+def test_fused_single_launch_all_masks(comm_dim, split):
+    """b200_dslash_apply_fused (pack + interior + boundary as one launch, or its pack + boundary and interior roles as two):
+    the interior role (every tile, face sites retire) and the boundary role (one thread per face site, corners owned by
+    the highest partitioned dimension) must cover every site exactly once and reproduce the periodic operator for all
+    15 partition masks"""
+    ops.check_partitioned(HostMem, twin_backend(), 8, 18, comm_dim, X=(4, 6, 4, 8), split=split)
 
 
 @pytest.mark.parametrize("prec,recon", [(4, 12), (2, 8)])
@@ -280,6 +282,25 @@ def test_batched_halo_argument_checks():
     outs, ins = [P.empty(), P.empty()], [f, P.to_dev(P.spinor(seed=3))]
     with pytest.raises(L.B200Error, match="own ghost slab"):
         D.ApplyWilson(outs, ins, P.U, 0.0, None, 0, 0, halo=halo, backend=be)
+    # the fused Dslash refuses pack arguments that do not describe its own input's faces
+    dst = [[None, None]] * 3 + [[halo.ghost[3][1], halo.ghost[3][0]]]
+    fused = dict(halo=halo, fused_dst=dst, block_counter=HostMem.empty(32))
+
+    def tampered(edit):  # the twin, with the pack arguments edited on the way in
+        class Backend:
+            def call(self, name, args, pack):
+                edit(pack._obj)
+                return be.call(name, args, pack)
+        return Backend()
+    D.ApplyWilson(outs[0], f, P.U, 0.0, None, 0, 0, backend=be, **fused)
+    with pytest.raises(L.B200Error, match="kernel must be AUTO"):
+        D.ApplyWilson(outs[0], f, P.U, 0.0, None, 0, 0, backend=be, kernel=L.KERNEL_INTERIOR, **fused)
+    with pytest.raises(L.B200Error, match=r"dst\[3\]\[1\] is NULL"):
+        D.ApplyWilson(outs[0], f, P.U, 0.0, None, 0, 0, backend=be, **dict(fused, fused_dst=dst[:3] + [[dst[3][0], None]]))
+    with pytest.raises(L.B200Error, match="different sequence numbers"):
+        D.ApplyWilson(outs[0], f, P.U, 0.0, None, 0, 0, backend=tampered(lambda p: setattr(p, "seq", p.seq + 1)), **fused)
+    with pytest.raises(L.B200Error, match="extents differ"):
+        D.ApplyWilson(outs[0], f, P.U, 0.0, None, 0, 0, backend=tampered(lambda p: p.X.__setitem__(0, 8)), **fused)
 
 
 @pytest.mark.parametrize("prec,recon,n_src,dims", [(8, 18, 3, (0, 0, 0, 1)), (4, 12, 8, (0, 1, 1, 1)), (2, 12, 4, (1, 1, 1, 1))])
@@ -331,7 +352,7 @@ def test_minimal_and_ragged_lattices(X):
     for d in range(4):
         mask = tuple(int(e == d) for e in range(4))
         if X[d] >= 4:
-            for split in (False, "tiles", "sites", "fused"):
+            for split in (False, "tiles", "sites", "fused", "fused_roles"):
                 ops.check_partitioned(HostMem, be, 4, 12, mask, X=X, xpay=True, split=split)
         else:
             from quda_b200 import lib as L
