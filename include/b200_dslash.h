@@ -325,6 +325,9 @@ typedef struct {
 } b200_solver_param;
 /* CG on MdagM x = b (x, b in the precise operator's precision; sloppy may equal precise) */
 int b200_invert_cg(b200_dirac *precise, b200_dirac *sloppy, const b200_spinor *x, const b200_spinor *b, b200_solver_param *param);
+/* BiCGStab on M x = b with the operator as given (the preconditioned system for the *pc types, the full one otherwise);
+ * same fields and precisions as b200_invert_cg, restarts after a breakdown are counted in reliable_updates */
+int b200_invert_bicgstab(b200_dirac *precise, b200_dirac *sloppy, const b200_spinor *x, const b200_spinor *b, b200_solver_param *param);
 
 const char *b200_last_error(void);
 int b200_abi_version(void);

@@ -28,7 +28,7 @@ namespace b200
 
   void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 
-  static int require_device()
+  int require_device()
   {
     int n = 0;
     cudaError_t e = cudaGetDeviceCount(&n);

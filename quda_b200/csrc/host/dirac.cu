@@ -400,45 +400,71 @@ namespace b200
         cudaEvent_t ev[8] = {};
         unsigned long long ring = 0;
       };
-      static Workspace &workspace(void *stream)
+      // CG's workspace (partials of kMaxVals per block, S_COUNT scalars) or BiCGStab's (4 per block, its own scalars)
+      static Workspace &workspace_of(std::map<void *, Workspace> &m, void *stream, int vals, int count)
       {
-        static std::map<void *, Workspace> m;
         Workspace &w = m[stream];
         if (!w.partials) {
-          cuda_ok(cudaMalloc(&w.partials, sizeof(double) * kBlocks * kMaxVals), "cudaMalloc(reduce)");
+          cuda_ok(cudaMalloc(&w.partials, sizeof(double) * kBlocks * vals), "cudaMalloc(reduce)");
           cuda_ok(cudaMalloc(&w.ticket, sizeof(unsigned)), "cudaMalloc(reduce)");
           cuda_ok(cudaMemset(w.ticket, 0, sizeof(unsigned)), "memset");
-          cuda_ok(cudaMalloc(&w.scalars, sizeof(double) * S_COUNT), "cudaMalloc(reduce)");
-          cuda_ok(cudaMemset(w.scalars, 0, sizeof(double) * S_COUNT), "memset");
-          cuda_ok(cudaHostAlloc(&w.host, sizeof(double) * 8 * S_COUNT, cudaHostAllocMapped), "cudaHostAlloc(reduce)");
+          cuda_ok(cudaMalloc(&w.scalars, sizeof(double) * count), "cudaMalloc(reduce)");
+          cuda_ok(cudaMemset(w.scalars, 0, sizeof(double) * count), "memset");
+          cuda_ok(cudaHostAlloc(&w.host, sizeof(double) * 8 * count, cudaHostAllocMapped), "cudaHostAlloc(reduce)");
           cuda_ok(cudaHostGetDevicePointer(&w.host_dev, w.host, 0), "cudaHostGetDevicePointer");
           for (auto &e : w.ev) cuda_ok(cudaEventCreateWithFlags(&e, cudaEventDisableTiming), "event");
         }
         return w;
       }
+      static Workspace &workspace(void *stream)
+      {
+        static std::map<void *, Workspace> m;
+        return workspace_of(m, stream, kMaxVals, S_COUNT);
+      }
+
+      // CG's finaliser: derives pAp / alpha or r2 / beta from the global sums v[0..NV) of one reduction
+      struct CgFinish {
+        static constexpr int kVals = kMaxVals, kCount = S_COUNT;
+        template <int NV> __device__ static void apply(double *S, const double *v, int fin)
+        {
+          const double v0 = v[0];
+          if (fin == FIN_PAP) {
+            S[S_PAP] = v0;
+            S[S_ALPHA] = S[S_R2] / v0;
+          } else if (fin == FIN_R2) {
+            const double old = S[S_R2];
+            S[S_R2_OLD] = old;
+            S[S_R2] = v0;
+            S[S_BETA] = v0 / old;
+          }
+          S[S_RAW0] = v0;
+          if (NV > 1) S[S_RAW1] = v[1];
+        }
+      };
 
       // Second stage of every reduction, run by the block that arrives last: sum the per-block partial sums in block
       // order (fixed -> bit-reproducible), all-reduce over the ranks through the NVLink mailboxes in rank order, derive
-      // the CG scalars and publish everything to the host mirror.
-      template <int NV>
+      // the solver's scalars (Fin: CgFinish or BicgFinish) and publish the scalar block to the host mirror.
+      template <int NV, typename Fin = CgFinish>
       __device__ void finish_reduction(const double *acc_block, double *partials, unsigned *ticket, double *S, double *host_out,
                                        int fin, ReducePeers peers)
       {
-        __shared__ double sh[kThreads][kMaxVals];
+        constexpr int MV = Fin::kVals;
+        __shared__ double sh[kThreads][MV];
         __shared__ bool is_last;
-        __shared__ double part[B200_MAX_RANKS][kMaxVals];
+        __shared__ double part[B200_MAX_RANKS][MV];
         const int t = threadIdx.x;
         if (t == 0) {
-          for (int i = 0; i < NV; i++) partials[blockIdx.x * kMaxVals + i] = acc_block[i];
+          for (int i = 0; i < NV; i++) partials[blockIdx.x * MV + i] = acc_block[i];
           __threadfence();
           is_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
         }
         __syncthreads();
         if (!is_last) return;
         __threadfence();
-        double a[kMaxVals] = {0, 0};
+        double a[MV] = {};
         for (int b = t; b < (int)gridDim.x; b += kThreads)
-          for (int i = 0; i < NV; i++) a[i] += __ldcg(partials + b * kMaxVals + i);
+          for (int i = 0; i < NV; i++) a[i] += __ldcg(partials + b * MV + i);
         for (int i = 0; i < NV; i++) sh[t][i] = a[i];
         __syncthreads();
         for (int s = kThreads / 2; s > 0; s >>= 1) {
@@ -476,20 +502,9 @@ namespace b200
             }
         }
         if (t == 0) {
-          const double v0 = sh[0][0];
-          if (fin == FIN_PAP) {
-            S[S_PAP] = v0;
-            S[S_ALPHA] = S[S_R2] / v0;
-          } else if (fin == FIN_R2) {
-            const double old = S[S_R2];
-            S[S_R2_OLD] = old;
-            S[S_R2] = v0;
-            S[S_BETA] = v0 / old;
-          }
-          S[S_RAW0] = v0;
-          if (NV > 1) S[S_RAW1] = sh[0][1];
+          Fin::template apply<NV>(S, sh[0], fin);
           if (host_out) {
-            for (int i = 0; i < S_COUNT; i++) host_out[i] = S[i];
+            for (int i = 0; i < Fin::kCount; i++) host_out[i] = S[i];
             __threadfence_system();
           }
           *ticket = 0;
@@ -586,6 +601,218 @@ namespace b200
       }
       __global__ void set_scalar_kernel(double *S, int idx, double v) { S[idx] = v; }
 
+      // ---- BiCGStab: its own device scalar block (complex scalars are (re, im) pairs) and finalisers
+      enum BicgScalar {
+        B_RHO = 0, B_ALPHA = 2, B_OMEGA = 4, B_BETA = 6, B_R2 = 8, B_STOP = 9,
+        B_DONE = 10,  // 1 once |r|^2 <= stop: every BiCGStab kernel after that returns at once, until the host clears it
+        B_BREAK = 11, // breakdown word (BRK_* bits): a zero divisor met while the residual was not 0
+        B_RAW = 12,   // the global sums of the last reduction, up to 4
+        B_COUNT = 16
+      };
+      enum BicgFinish { BF_RAW = 0, BF_RHO = 1, BF_ALPHA = 2, BF_OMEGA = 3, BF_BETA = 4 };
+      enum { BRK_ALPHA = 1, BRK_OMEGA = 2, BRK_BETA = 4 };
+
+      // rounded products: no FMA contraction, so that (a + ib) / (a + ib) is exactly 1 on the device and on the host
+      __host__ __device__ inline double mul_rn(double a, double b)
+      {
+#ifdef __CUDA_ARCH__
+        return __dmul_rn(a, b);
+#else
+        return a * b;
+#endif
+      }
+      // q = n / d, or 0 if d == 0 (returns false then)
+      __host__ __device__ inline bool cdiv(double *q, double nr, double ni, double dr, double di)
+      {
+        const double den = mul_rn(dr, dr) + mul_rn(di, di);
+        if (den == 0.0) {
+          q[0] = q[1] = 0.0;
+          return false;
+        }
+        q[0] = (mul_rn(nr, dr) + mul_rn(ni, di)) / den;
+        q[1] = (mul_rn(ni, dr) - mul_rn(nr, di)) / den;
+        return true;
+      }
+      __host__ __device__ inline void cmul(double *q, double ar, double ai, double br, double bi)
+      {
+        const double re = mul_rn(ar, br) - mul_rn(ai, bi), im = mul_rn(ar, bi) + mul_rn(ai, br);
+        q[0] = re;
+        q[1] = im;
+      }
+      // a zero divisor is a breakdown unless the residual the step leaves behind is 0 (that is convergence)
+      __host__ __device__ inline void breakdown(double *S, int bit, double r2_left)
+      {
+        if (r2_left != 0.0) S[B_BREAK] = (double)((int)S[B_BREAK] | bit);
+      }
+      // Derive BiCGStab's scalars from the global sums in S[B_RAW..]: on the device in the last block of a reduction, or on
+      // the host after the host all-reduce (no NVLink mailboxes).
+      //   BF_RHO    v = <r0, r>                 rho <- v
+      //   BF_ALPHA  v = <r0, v>                 alpha = rho / v            (0 if v == 0)
+      //   BF_OMEGA  v = <t, s>, |t|^2, |s|^2    omega = <t, s> / |t|^2     (0 if |t|^2 == 0; s is then left as r)
+      //   BF_BETA   v = <r0, r>, |r|^2          beta = (v / rho)(alpha / omega) (0 if omega or rho is 0), rho <- v, r2 <- |r|^2
+      __host__ __device__ inline void bicg_scalars(double *S, int fin)
+      {
+        const double *v = S + B_RAW;
+        if (fin == BF_RHO) {
+          S[B_RHO] = v[0];
+          S[B_RHO + 1] = v[1];
+        } else if (fin == BF_ALPHA) {
+          if (!cdiv(S + B_ALPHA, S[B_RHO], S[B_RHO + 1], v[0], v[1])) breakdown(S, BRK_ALPHA, S[B_R2]);
+        } else if (fin == BF_OMEGA) {
+          if (v[2] == 0.0) {
+            S[B_OMEGA] = S[B_OMEGA + 1] = 0.0;
+            breakdown(S, BRK_OMEGA, v[3]);
+          } else {
+            S[B_OMEGA] = v[0] / v[2];
+            S[B_OMEGA + 1] = v[1] / v[2];
+          }
+        } else if (fin == BF_BETA) {
+          double q[2], a[2];
+          const bool ok = cdiv(q, v[0], v[1], S[B_RHO], S[B_RHO + 1]) && cdiv(a, S[B_ALPHA], S[B_ALPHA + 1], S[B_OMEGA], S[B_OMEGA + 1]);
+          if (ok) {
+            cmul(S + B_BETA, q[0], q[1], a[0], a[1]);
+          } else {
+            S[B_BETA] = S[B_BETA + 1] = 0.0;
+            breakdown(S, BRK_BETA, v[2]);
+          }
+          S[B_RHO] = v[0];
+          S[B_RHO + 1] = v[1];
+          S[B_R2] = v[2];
+          if (v[2] <= S[B_STOP]) S[B_DONE] = 1.0;
+        }
+      }
+      struct BicgFinishOp {
+        static constexpr int kVals = 4, kCount = B_COUNT;
+        template <int NV> __device__ static void apply(double *S, const double *v, int fin)
+        {
+          for (int i = 0; i < NV; i++) S[B_RAW + i] = v[i];
+          bicg_scalars(S, fin);
+        }
+      };
+
+      template <typename T> struct Cplx;
+      template <> struct Cplx<double> {
+        using type = double2;
+      };
+      template <> struct Cplx<float> {
+        using type = float2;
+      };
+
+      // The five streaming kernels of a BiCGStab iteration walk the field as complex numbers: in both native orders (fp64
+      // planes of 2 reals, fp32 planes of 4) the real index 2c + re/im keeps each pair adjacent, so element pair i is one
+      // complex component.  n is the number of complex elements.  Every kernel returns at once when S[B_DONE] is set.
+      template <int NV> __device__ __forceinline__ void bicg_finish(const double (&acc)[NV], const ReduceArgs &ra)
+      {
+        __shared__ double wb[kThreads / 32];
+        double s[NV];
+#pragma unroll
+        for (int i = 0; i < NV; i++) s[i] = block_sum(acc[i], wb);
+        finish_reduction<NV, BicgFinishOp>(s, ra.partials, ra.ticket, ra.S, ra.host_out, ra.fin, ra.peers);
+      }
+
+      // K1 (and the rho (re)computation): <a, b> = sum conj(a) b
+      template <typename T>
+      __global__ void __launch_bounds__(kThreads) bicg_cdot_kernel(const T *__restrict__ a_, const T *__restrict__ b_, size_t n, ReduceArgs ra)
+      {
+        using C2 = typename Cplx<T>::type;
+        if (ra.S[B_DONE] != 0.0) return;
+        const C2 *a = reinterpret_cast<const C2 *>(a_), *b = reinterpret_cast<const C2 *>(b_);
+        double acc[2] = {0, 0};
+        for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+          const C2 x = a[i], y = b[i];
+          acc[0] += (double)x.x * y.x + (double)x.y * y.y;
+          acc[1] += (double)x.x * y.y - (double)x.y * y.x;
+        }
+        bicg_finish<2>(acc, ra);
+      }
+      // K2: s = r - alpha v, in place in r
+      template <typename T>
+      __global__ void __launch_bounds__(kThreads) bicg_update_s_kernel(T *__restrict__ r_, const T *__restrict__ v_, size_t n, const double *__restrict__ S)
+      {
+        using C2 = typename Cplx<T>::type;
+        if (S[B_DONE] != 0.0) return;
+        const double ar = S[B_ALPHA], ai = S[B_ALPHA + 1];
+        C2 *r = reinterpret_cast<C2 *>(r_);
+        const C2 *v = reinterpret_cast<const C2 *>(v_);
+        for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+          const C2 x = v[i], y = r[i];
+          C2 o;
+          o.x = (T)((double)y.x - (ar * x.x - ai * x.y));
+          o.y = (T)((double)y.y - (ar * x.y + ai * x.x));
+          r[i] = o;
+        }
+      }
+      // K3: <t, s>, |t|^2, |s|^2
+      template <typename T>
+      __global__ void __launch_bounds__(kThreads) bicg_ts_kernel(const T *__restrict__ t_, const T *__restrict__ s_, size_t n, ReduceArgs ra)
+      {
+        using C2 = typename Cplx<T>::type;
+        if (ra.S[B_DONE] != 0.0) return;
+        const C2 *t = reinterpret_cast<const C2 *>(t_), *s = reinterpret_cast<const C2 *>(s_);
+        double acc[4] = {0, 0, 0, 0};
+        for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+          const C2 x = t[i], y = s[i];
+          acc[0] += (double)x.x * y.x + (double)x.y * y.y;
+          acc[1] += (double)x.x * y.y - (double)x.y * y.x;
+          acc[2] += (double)x.x * x.x + (double)x.y * x.y;
+          acc[3] += (double)y.x * y.x + (double)y.y * y.y;
+        }
+        bicg_finish<4>(acc, ra);
+      }
+      // K4: x += alpha p + omega s ; r = s - omega t (r holds s) ; <r0, r>, |r|^2 of the stored r
+      template <typename T>
+      __global__ void __launch_bounds__(kThreads) bicg_update_xr_kernel(T *__restrict__ x_, T *__restrict__ r_, const T *__restrict__ p_,
+                                                                        const T *__restrict__ t_, const T *__restrict__ r0_, size_t n, ReduceArgs ra)
+      {
+        using C2 = typename Cplx<T>::type;
+        const double *S = ra.S;
+        if (S[B_DONE] != 0.0) return;
+        const double ar = S[B_ALPHA], ai = S[B_ALPHA + 1], wr = S[B_OMEGA], wi = S[B_OMEGA + 1];
+        C2 *x = reinterpret_cast<C2 *>(x_), *r = reinterpret_cast<C2 *>(r_);
+        const C2 *p = reinterpret_cast<const C2 *>(p_), *t = reinterpret_cast<const C2 *>(t_), *r0 = reinterpret_cast<const C2 *>(r0_);
+        double acc[3] = {0, 0, 0};
+        for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+          const C2 pv = p[i], sv = r[i], tv = t[i], xv = x[i], hv = r0[i];
+          C2 xo, ro;
+          xo.x = (T)((double)xv.x + (ar * pv.x - ai * pv.y) + (wr * sv.x - wi * sv.y));
+          xo.y = (T)((double)xv.y + (ar * pv.y + ai * pv.x) + (wr * sv.y + wi * sv.x));
+          ro.x = (T)((double)sv.x - (wr * tv.x - wi * tv.y));
+          ro.y = (T)((double)sv.y - (wr * tv.y + wi * tv.x));
+          x[i] = xo;
+          r[i] = ro;
+          acc[0] += (double)hv.x * ro.x + (double)hv.y * ro.y;
+          acc[1] += (double)hv.x * ro.y - (double)hv.y * ro.x;
+          acc[2] += (double)ro.x * ro.x + (double)ro.y * ro.y;
+        }
+        bicg_finish<3>(acc, ra);
+      }
+      // K5: p = r + beta (p - omega v)
+      template <typename T>
+      __global__ void __launch_bounds__(kThreads) bicg_update_p_kernel(T *__restrict__ p_, const T *__restrict__ r_, const T *__restrict__ v_,
+                                                                       size_t n, const double *__restrict__ S)
+      {
+        using C2 = typename Cplx<T>::type;
+        if (S[B_DONE] != 0.0) return;
+        const double br = S[B_BETA], bi = S[B_BETA + 1], wr = S[B_OMEGA], wi = S[B_OMEGA + 1];
+        C2 *p = reinterpret_cast<C2 *>(p_);
+        const C2 *r = reinterpret_cast<const C2 *>(r_), *v = reinterpret_cast<const C2 *>(v_);
+        for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+          const C2 pv = p[i], rv = r[i], vv = v[i];
+          const double dr = pv.x - (wr * vv.x - wi * vv.y), di = pv.y - (wr * vv.y + wi * vv.x);
+          C2 o;
+          o.x = (T)((double)rv.x + (br * dr - bi * di));
+          o.y = (T)((double)rv.y + (br * di + bi * dr));
+          p[i] = o;
+        }
+      }
+      struct BicgScalars {
+        double s[B_COUNT];
+      };
+      __global__ void set_bicg_scalars_kernel(double *S, BicgScalars v)
+      {
+        if (threadIdx.x < B_COUNT) S[threadIdx.x] = v.s[threadIdx.x];
+      }
+
       static void check_pair(const ColorSpinorField &x, const ColorSpinorField &y)
       {
         if (x.Length() != y.Length()) throw Error("blas: operands differ in length");
@@ -613,20 +840,20 @@ namespace b200
         Workspace *w;
         int slot;
       };
-      static ReduceArgs reduce_args(const Exec &ex, int fin, Pending &pend)
+      static ReduceArgs reduce_args(const Exec &ex, Workspace &w, int count, int fin, Pending &pend)
       {
-        Workspace &w = workspace(ex.stream);
         pend.w = &w;
         pend.slot = (int)(w.ring++ & 7);
         ReduceArgs ra;
         ra.partials = w.partials;
         ra.ticket = w.ticket;
         ra.S = w.scalars;
-        ra.host_out = w.host_dev + pend.slot * S_COUNT;
+        ra.host_out = w.host_dev + pend.slot * count;
         ra.fin = fin;
         ra.peers = peers_of(ex.comm);
         return ra;
       }
+      static ReduceArgs reduce_args(const Exec &ex, int fin, Pending &pend) { return reduce_args(ex, workspace(ex.stream), S_COUNT, fin, pend); }
       static void mark(const Exec &ex, const Pending &p) { cuda_ok(cudaEventRecord(p.w->ev[p.slot], cs(ex.stream)), "record"); }
       // wait for a reduction launched earlier and return the host mirror of the device scalars as of that launch;
       // multi-rank sums without NVLink mailboxes go through the host callback here
@@ -773,6 +1000,129 @@ namespace b200
         cuda_ok(cudaGetLastError(), "blas launch");
         g_flops += 2 * (long long)n;
       }
+
+      // ---- BiCGStab iteration pieces (used by invertBiCGStab below); all operands share the sloppy precision
+      static Workspace &bicg_workspace(void *stream)
+      {
+        static std::map<void *, Workspace> m;
+        return workspace_of(m, stream, BicgFinishOp::kVals, B_COUNT);
+      }
+      // host mirror of BiCGStab's scalar block as of a reduction launched earlier (waits for it)
+      static const double *bicg_await(const Pending &p)
+      {
+        cuda_ok(cudaEventSynchronize(p.w->ev[p.slot]), "event sync");
+        return p.w->host + p.slot * B_COUNT;
+      }
+      static void bicg_set(const Exec &ex, int idx, double v)
+      {
+        set_scalar_kernel<<<1, 1, 0, cs(ex.stream)>>>(bicg_workspace(ex.stream).scalars, idx, v);
+        cuda_ok(cudaGetLastError(), "scalar launch");
+      }
+      static void bicg_set_all(const Exec &ex, const BicgScalars &s)
+      {
+        set_bicg_scalars_kernel<<<1, 32, 0, cs(ex.stream)>>>(bicg_workspace(ex.stream).scalars, s);
+        cuda_ok(cudaGetLastError(), "scalar launch");
+      }
+      static void bicg_check(const ColorSpinorField &a, const ColorSpinorField &b)
+      {
+        check_pair(a, b);
+        if (a.precision != b.precision) throw Error("blas: operands differ in precision");
+      }
+      // Launch one BiCGStab reduction of nv sums with finaliser fin.  With NVLink mailboxes, or on one rank, the last block
+      // derives the scalars on the device and nothing waits.  With the host all-reduce the kernel only publishes its local
+      // sums; all nv of them go through the callback, the host derives the scalars with the same code, writes the whole
+      // block back to the device and into the mirror slot, so bicg_await() reads the same thing in both cases.
+      template <typename Launch>
+      static Pending bicg_reduce(const Exec &ex, int nv, int fin, bool host_ar, int &syncs, Launch &&launch)
+      {
+        Pending pend {};
+        const ReduceArgs ra = reduce_args(ex, bicg_workspace(ex.stream), B_COUNT, host_ar ? (int)BF_RAW : fin, pend);
+        launch(ra);
+        cuda_ok(cudaGetLastError(), "blas launch");
+        mark(ex, pend);
+        if (host_ar) {
+          BicgScalars s;
+          memcpy(s.s, bicg_await(pend), sizeof(s.s));
+          syncs++;
+          ex.comm->allreduce_sum(s.s + B_RAW, nv, ex.comm->user);
+          bicg_scalars(s.s, fin);
+          bicg_set_all(ex, s);
+          memcpy(pend.w->host + pend.slot * B_COUNT, s.s, sizeof(s.s));
+        }
+        return pend;
+      }
+      // <a, b> (K1 with BF_ALPHA; rho = <r0, r> with BF_RHO)
+      static Pending bicg_cdot(const ColorSpinorField &a, const ColorSpinorField &b, int fin, const Exec &ex, bool host_ar, int &syncs)
+      {
+        bicg_check(a, b);
+        const size_t n = a.Length() / 2;
+        g_flops += 8 * (long long)n;
+        return bicg_reduce(ex, 2, fin, host_ar, syncs, [&](const ReduceArgs &ra) {
+          if (a.precision == 8)
+            bicg_cdot_kernel<double><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((const double *)a.v, (const double *)b.v, n, ra);
+          else
+            bicg_cdot_kernel<float><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((const float *)a.v, (const float *)b.v, n, ra);
+        });
+      }
+      // K2
+      static void bicg_update_s(ColorSpinorField &r, const ColorSpinorField &v, const Exec &ex)
+      {
+        bicg_check(r, v);
+        const size_t n = r.Length() / 2;
+        const double *S = bicg_workspace(ex.stream).scalars;
+        if (r.precision == 8)
+          bicg_update_s_kernel<double><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((double *)r.v, (const double *)v.v, n, S);
+        else
+          bicg_update_s_kernel<float><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((float *)r.v, (const float *)v.v, n, S);
+        cuda_ok(cudaGetLastError(), "blas launch");
+        g_flops += 8 * (long long)n;
+      }
+      // K3
+      static Pending bicg_ts(const ColorSpinorField &t, const ColorSpinorField &s, const Exec &ex, bool host_ar, int &syncs)
+      {
+        bicg_check(t, s);
+        const size_t n = t.Length() / 2;
+        g_flops += 16 * (long long)n;
+        return bicg_reduce(ex, 4, BF_OMEGA, host_ar, syncs, [&](const ReduceArgs &ra) {
+          if (t.precision == 8)
+            bicg_ts_kernel<double><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((const double *)t.v, (const double *)s.v, n, ra);
+          else
+            bicg_ts_kernel<float><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((const float *)t.v, (const float *)s.v, n, ra);
+        });
+      }
+      // K4
+      static Pending bicg_update_xr(ColorSpinorField &x, ColorSpinorField &r, const ColorSpinorField &p, const ColorSpinorField &t,
+                                    const ColorSpinorField &r0, const Exec &ex, bool host_ar, int &syncs)
+      {
+        bicg_check(x, r);
+        bicg_check(x, p);
+        bicg_check(x, t);
+        bicg_check(x, r0);
+        const size_t n = x.Length() / 2;
+        g_flops += 36 * (long long)n;
+        return bicg_reduce(ex, 3, BF_BETA, host_ar, syncs, [&](const ReduceArgs &ra) {
+          if (x.precision == 8)
+            bicg_update_xr_kernel<double><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(
+              (double *)x.v, (double *)r.v, (const double *)p.v, (const double *)t.v, (const double *)r0.v, n, ra);
+          else
+            bicg_update_xr_kernel<float><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(
+              (float *)x.v, (float *)r.v, (const float *)p.v, (const float *)t.v, (const float *)r0.v, n, ra);
+        });
+      }
+      // K5
+      static void bicg_update_p(ColorSpinorField &p, const ColorSpinorField &r, const ColorSpinorField &v, const Exec &ex)
+      {
+        bicg_check(p, r);
+        bicg_check(p, v);
+        const size_t n = p.Length() / 2;
+        const double *S = bicg_workspace(ex.stream).scalars;
+        if (p.precision == 8)
+          bicg_update_p_kernel<double><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((double *)p.v, (const double *)r.v, (const double *)v.v, n, S);
+        else
+          bicg_update_p_kernel<float><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((float *)p.v, (const float *)r.v, (const float *)v.v, n, S);
+        cuda_ok(cudaGetLastError(), "blas launch");
+        g_flops += 16 * (long long)n;
+      }
     } // namespace blas
 
     // ------------------------------------------------------------------ the even-odd operator
@@ -821,6 +1171,12 @@ namespace b200
     void Dirac::hop(ColorSpinorField &out, const ColorSpinorField &in, int parity, Fuse f, const ColorSpinorField *x, double k) const
     {
       need_single_parity(in, out);
+      if (x && k == 0.0) {
+        // x + 0 D in: the launch ABI reads a == 0 as "no x term", so the hop is skipped rather than issued (kappa = 0)
+        if (f == Fuse::A) site(out, *x, parity, false);
+        else blas::copy(out, *x, exec());
+        return;
+      }
       const ColorSpinorField &xf = x ? *x : in;
       const double a = x ? k : 0.0;
       if (term == SiteTerm::Identity || f == Fuse::None) {
@@ -872,7 +1228,7 @@ namespace b200
       if (!schur) {
         // out_p = A_p in_p - kappa D in_{1-p}
         need_full(out, in);
-        const bool one_launch = term != SiteTerm::Twist && !(comm && comm->partitioned());
+        const bool one_launch = term != SiteTerm::Twist && !(comm && comm->partitioned()) && kappa != 0.0;
         if (one_launch) { // both parities in one launch (full-field kernel)
           if (term == SiteTerm::Identity)
             ApplyWilson(out, in, *gauge, -kappa, in, QUDA_INVALID_PARITY, dagger, commDim, comm, stream);
@@ -1125,6 +1481,169 @@ namespace b200
       copy(x, y, ex);
       // true residual
       mat.MdagM(tmp, x);
+      copy(r, b, ex);
+      const double tr2 = axpyNorm(-1.0, tmp, r, ex);
+      syncs++;
+      cuda_ok(cudaStreamSynchronize(cs(ex.stream)), "sync");
+      if (halo_timed_out(ex.comm, ex.stream)) throw Error("a halo wait timed out during the solve: the result is not valid");
+      param.iter = k;
+      param.true_res = std::sqrt(tr2 / b2);
+      param.host_syncs = syncs;
+      param.secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+      const long long nds = mat.DslashApplications() + matSloppy.DslashApplications() - ds0;
+      const double fl = (double)(blas::flops() - flops0) + (double)nds * 1320.0 * x.VolumeCB();
+      param.gflops = fl / param.secs * 1e-9;
+    }
+
+    // ------------------------------------------------------------------ BiCGStab (M x = b) with reliable updates
+    // The reference's recurrence and reliable-update criterion (lib/inv_bicgstab_quda.cpp:71-80, 187-355) with CG's
+    // structure: rho, alpha, omega, beta and |r|^2 live on the device (blas::bicg_scalars, run by the reduction finalisers),
+    // one iteration is v = M p, K1..K5 and t = M s around them, and the host reads |r|^2 and the breakdown word of
+    // iteration k - 1 while the GPU runs iteration k.  When |r|^2 reaches the stopping value the K4 finaliser sets B_DONE
+    // and the kernels of the iteration already queued behind it return at once, so the solution is that of the iteration
+    // the host reports.
+    // A late reliable update replaces r (and rho = <r0, r>) after iteration k has run and keeps p.  The recursion stays
+    // consistent because x and r are only ever changed together, x += alpha p + omega s against r -= alpha M p + omega M s,
+    // so r = b - M x holds for any search direction p; keeping p only perturbs the bi-orthogonality of the directions by
+    // the drift r_true - r_sloppy, and rho is recomputed so that alpha = rho / <r0, M p> and the next beta refer to the
+    // residual the recursion now carries.  A restart after a breakdown additionally sets r0 = p = r.
+    void invertBiCGStab(const Dirac &mat, const Dirac &matSloppy, ColorSpinorField &x, const ColorSpinorField &b, SolverParam &param)
+    {
+      using namespace blas;
+      const Exec ex = mat.exec();
+      if (matSloppy.Stream() != mat.Stream()) throw Error("precise and sloppy operators must share a stream");
+      const auto t0 = std::chrono::steady_clock::now();
+      const long long flops0 = blas::flops();
+      const long long ds0 = mat.DslashApplications() + matSloppy.DslashApplications();
+      const bool mixed = (&mat != &matSloppy);
+      const int sp = matSloppy.Precision();
+      if (x.precision != mat.Precision() || b.precision != mat.Precision()) throw Error("x and b must have the precise operator's precision");
+      if (sp != 8 && sp != 4) throw Error("the sloppy operator must be double or single precision");
+      if (mixed && sp > x.precision) throw Error("the sloppy operator is more precise than the precise one");
+      const bool host_ar = host_allreduce(ex);
+      int syncs = 0;
+
+      Scratch r_s(ex.stream, x.X, x.precision, x.n_parity), y_s(ex.stream, x.X, x.precision, x.n_parity),
+        tmp_s(ex.stream, x.X, x.precision, x.n_parity);
+      ColorSpinorField &r = r_s.f;     // high-precision residual
+      ColorSpinorField &y = y_s.f;     // high-precision accumulated solution
+      ColorSpinorField &tmp = tmp_s.f;
+      const bool same_prec = sp == x.precision;
+      Scratch xS_s(ex.stream, x.X, sp, x.n_parity), p_s(ex.stream, x.X, sp, x.n_parity), v_s(ex.stream, x.X, sp, x.n_parity),
+        t_s(ex.stream, x.X, sp, x.n_parity), r0_s(ex.stream, x.X, sp, x.n_parity);
+      std::unique_ptr<Scratch> rS_s;
+      if (!same_prec) rS_s.reset(new Scratch(ex.stream, x.X, sp, x.n_parity));
+      ColorSpinorField rS = same_prec ? r : rS_s->f; // sloppy residual; holds s between K2 and K4
+      ColorSpinorField &xS = xS_s.f, &p = p_s.f, &v = v_s.f, &t = t_s.f, &r0 = r0_s.f;
+
+      const double b2 = norm2(b, ex);
+      syncs++;
+      if (b2 == 0.0) {
+        zero(x, ex);
+        param.iter = 0;
+        param.true_res = 0.0;
+        return;
+      }
+      const double stop = param.tol * param.tol * b2;
+      double r2 = 0.0, maxrr = 0.0;
+      int k = 0;
+      param.reliable_updates = 0;
+
+      // y += x_sloppy, r = b - M y in the precise operator, r_sloppy = r; clears the device flags
+      auto true_residual = [&]() {
+        if (same_prec) {
+          axpy(1.0, xS, y, ex);
+        } else {
+          copy(tmp, xS, ex);
+          axpy(1.0, tmp, y, ex);
+        }
+        zero(xS, ex);
+        mat.M(tmp, y);
+        copy(r, b, ex);
+        r2 = axpyNorm(-1.0, tmp, r, ex);
+        syncs++;
+        if (!same_prec) copy(rS, r, ex);
+        bicg_set(ex, B_R2, r2);
+        bicg_set(ex, B_DONE, 0.0);
+        bicg_set(ex, B_BREAK, 0.0);
+        maxrr = std::sqrt(r2);
+      };
+      auto recompute_rho = [&]() { bicg_cdot(r0, rS, BF_RHO, ex, host_ar, syncs); };
+
+      // r = b - M x, r0 = p = r, rho = <r0, r>
+      copy(y, x, ex);
+      mat.M(tmp, x);
+      copy(r, b, ex);
+      r2 = axpyNorm(-1.0, tmp, r, ex);
+      syncs++;
+      maxrr = std::sqrt(r2);
+      if (!same_prec) copy(rS, r, ex);
+      zero(xS, ex);
+      copy(r0, rS, ex);
+      copy(p, rS, ex);
+      BicgScalars s0 {};
+      s0.s[B_R2] = r2;
+      s0.s[B_STOP] = stop;
+      bicg_set_all(ex, s0);
+      recompute_rho();
+      bool done = r2 <= stop;
+
+      // convergence / reliable-update / restart decision on the scalar block after iteration j; true if r was replaced
+      auto decide = [&](const double *S, int j) {
+        r2 = S[B_R2];
+        const bool converged = S[B_DONE] != 0.0, broke = S[B_BREAK] != 0.0;
+        if (converged) k = j; // the iteration queued after j returned at once
+        const double rNorm = std::sqrt(r2);
+        if (rNorm > maxrr) maxrr = rNorm;
+        if (broke) { // restart from the true residual with a new shadow residual
+          true_residual();
+          copy(r0, rS, ex);
+          copy(p, rS, ex);
+        } else if (!same_prec && (converged || rNorm < param.delta * maxrr)) {
+          true_residual(); // reliable update: p is kept
+        } else {
+          done = converged;
+          return false;
+        }
+        recompute_rho();
+        param.reliable_updates++;
+        done = r2 <= stop;
+        return true;
+      };
+
+      Pending prev {};
+      bool have_prev = false;
+      while (!done && k < param.maxiter) {
+        matSloppy.M(v, p);
+        bicg_cdot(r0, v, BF_ALPHA, ex, host_ar, syncs);    // K1
+        bicg_update_s(rS, v, ex);                           // K2
+        matSloppy.M(t, rS);
+        bicg_ts(t, rS, ex, host_ar, syncs);                 // K3
+        Pending p4 = bicg_update_xr(xS, rS, p, t, r0, ex, host_ar, syncs); // K4
+        bicg_update_p(p, rS, v, ex);                        // K5
+        k++;
+        if (host_ar) { // every reduction has already been waited for
+          decide(bicg_await(p4), k);
+          continue;
+        }
+        bool replaced = false;
+        if (have_prev) {
+          replaced = decide(bicg_await(prev), k - 1);
+          syncs++;
+        }
+        // after a replacement the pending scalars belong to the recursion before it
+        have_prev = !replaced;
+        prev = p4;
+      }
+      // x = y + x_sloppy
+      if (same_prec) {
+        axpy(1.0, xS, y, ex);
+      } else {
+        copy(tmp, xS, ex);
+        axpy(1.0, tmp, y, ex);
+      }
+      copy(x, y, ex);
+      mat.M(tmp, x);
       copy(r, b, ex);
       const double tr2 = axpyNorm(-1.0, tmp, r, ex);
       syncs++;

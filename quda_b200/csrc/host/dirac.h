@@ -226,6 +226,10 @@ namespace b200
     // Solve MdagM x = b.  `mat` is the high-precision operator, `matSloppy` the low-precision one (may be the same object).
     void invertCG(const Dirac &mat, const Dirac &matSloppy, ColorSpinorField &x, const ColorSpinorField &b, SolverParam &param);
 
+    // ---- BiCGStab on M itself (behaviour of lib/inv_bicgstab_quda.cpp): the same precise / sloppy split and SolverParam;
+    // restarts after a breakdown are counted in reliable_updates
+    void invertBiCGStab(const Dirac &mat, const Dirac &matSloppy, ColorSpinorField &x, const ColorSpinorField &b, SolverParam &param);
+
     // true if a halo wait gave up since the last call (clears the flag); the C entry points turn it into an error
     bool halo_timed_out(CommContext *comm, void *stream);
 

@@ -7,6 +7,7 @@
 namespace b200
 {
   int set_error(int code, const char *fmt, ...);
+  int require_device();
 }
 
 using namespace b200::host;
@@ -187,32 +188,48 @@ int b200_dirac_reconstruct(b200_dirac *h, const b200_spinor *x, const b200_spino
   });
 }
 
+using Solver = void (*)(const Dirac &, const Dirac &, ColorSpinorField &, const ColorSpinorField &, SolverParam &);
+
+// comm mirroring and parameter marshaling shared by the solver entry points
+static void invert(Solver solve, b200_dirac *precise, b200_dirac *sloppy, const b200_spinor *x, const b200_spinor *b,
+                   b200_solver_param *param)
+{
+  if (!sloppy) sloppy = precise;
+  pull_comm(precise);
+  if (sloppy != precise) {
+    // a partitioned mixed-precision solve needs one halo context per precision (the ghost buffers differ in size);
+    // both advance in lock step on every rank because all ranks execute the same operator sequence
+    if (precise->has_comm != sloppy->has_comm) throw Error("precise / sloppy operators disagree on partitioning");
+    pull_comm(sloppy);
+  }
+  auto xf = wrap(precise, x), bf = wrap(precise, b);
+  SolverParam sp;
+  sp.tol = param->tol;
+  sp.maxiter = param->maxiter;
+  sp.delta = param->delta > 0 ? param->delta : 0.1;
+  solve(*precise->op, *sloppy->op, xf, bf, sp);
+  param->iter = sp.iter;
+  param->reliable_updates = sp.reliable_updates;
+  param->true_res = sp.true_res;
+  param->secs = sp.secs;
+  param->gflops = sp.gflops;
+  param->host_syncs = sp.host_syncs;
+  push_comm(precise);
+  if (sloppy != precise) push_comm(sloppy);
+}
+
+int b200_invert_bicgstab(b200_dirac *precise, b200_dirac *sloppy, const b200_spinor *x, const b200_spinor *b, b200_solver_param *param)
+{
+  if (!precise || !param) return b200::set_error(B200_ERR_INVALID, "b200_invert_bicgstab: null argument");
+  if (int rc = b200::require_device()) return rc;
+  return guarded([&] { invert(invertBiCGStab, precise, sloppy, x, b, param); });
+}
+
 int b200_invert_cg(b200_dirac *precise, b200_dirac *sloppy, const b200_spinor *x, const b200_spinor *b, b200_solver_param *param)
 {
   return guarded([&] {
     if (!precise || !param) throw Error("b200_invert_cg: null argument");
-    if (!sloppy) sloppy = precise;
-    pull_comm(precise);
-    if (sloppy != precise) {
-      // a partitioned mixed-precision solve needs one halo context per precision (the ghost buffers differ in size);
-      // both advance in lock step on every rank because all ranks execute the same operator sequence
-      if (precise->has_comm != sloppy->has_comm) throw Error("precise / sloppy operators disagree on partitioning");
-      pull_comm(sloppy);
-    }
-    auto xf = wrap(precise, x), bf = wrap(precise, b);
-    SolverParam sp;
-    sp.tol = param->tol;
-    sp.maxiter = param->maxiter;
-    sp.delta = param->delta > 0 ? param->delta : 0.1;
-    invertCG(*precise->op, *sloppy->op, xf, bf, sp);
-    param->iter = sp.iter;
-    param->reliable_updates = sp.reliable_updates;
-    param->true_res = sp.true_res;
-    param->secs = sp.secs;
-    param->gflops = sp.gflops;
-    param->host_syncs = sp.host_syncs;
-    push_comm(precise);
-    if (sloppy != precise) push_comm(sloppy);
+    invert(invertCG, precise, sloppy, x, b, param);
   });
 }
 }

@@ -76,3 +76,17 @@ def invert_cg(precise, sloppy, x, b, tol=1e-10, maxiter=10000, delta=0.1):
     xd, bd = x.desc(), b.desc()
     L.check(precise.lib.b200_invert_cg(precise.h, sloppy.h if sloppy is not None else None, C.byref(xd), C.byref(bd), C.byref(p)))
     return p
+
+
+def invert_bicgstab(precise, sloppy, x, b, tol=1e-10, maxiter=10000, delta=0.1):
+    """BiCGStab on M x = b with the operator as given (lib/inv_bicgstab_quda.cpp); returns the filled SolverParam.
+    x and b must have the precise operator's precision (the C ABI reads them in that precision)."""
+    for name, f in (("x", x), ("b", b)):
+        if f.prec != precise.prec:
+            raise L.B200Error(f"invert_bicgstab: {name} has precision {f.prec}, the precise operator {precise.prec}")
+    p = L.SolverParam()
+    p.tol, p.maxiter, p.delta = tol, maxiter, delta
+    xd, bd = x.desc(), b.desc()
+    L.check(precise.lib.b200_invert_bicgstab(precise.h, sloppy.h if sloppy is not None else None, C.byref(xd), C.byref(bd),
+                                             C.byref(p)))
+    return p

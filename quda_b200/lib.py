@@ -152,6 +152,8 @@ def load():
         lib.b200_dirac_reconstruct.restype = C.c_int
         lib.b200_invert_cg.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(Spinor), C.POINTER(Spinor), C.POINTER(SolverParam)]
         lib.b200_invert_cg.restype = C.c_int
+        lib.b200_invert_bicgstab.argtypes = lib.b200_invert_cg.argtypes
+        lib.b200_invert_bicgstab.restype = C.c_int
         lib.b200_comm_check.argtypes, lib.b200_comm_check.restype = [C.POINTER(Comm), C.c_void_p], C.c_int
         if lib.b200_abi_version() != ABI_VERSION:
             raise B200Error("libquda_b200.so ABI version mismatch")
@@ -170,5 +172,5 @@ EXPORTED_SYMBOLS = ["b200_dslash_apply", "b200_dslash_apply_fused", "b200_dslash
                     "b200_copy_spinor", "b200_copy_gauge", "b200_copy_clover", "b200_comm_alloc", "b200_comm_free", "b200_ipc_get_handle", "b200_ipc_open_handle",
                     "b200_ipc_close_handle", "b200_comm_copy",
                     "b200_dirac_create", "b200_dirac_set_twist", "b200_dirac_destroy", "b200_dirac_apply", "b200_dirac_prepare",
-                    "b200_dirac_reconstruct", "b200_invert_cg", "b200_comm_check",
+                    "b200_dirac_reconstruct", "b200_invert_cg", "b200_invert_bicgstab", "b200_comm_check",
                     "b200_last_error", "b200_abi_version", "b200_launch_count", "b200_reset_launch_count"]
