@@ -6,6 +6,7 @@
 #include <cstring>
 #include <map>
 #include <memory>
+#include <type_traits>
 #include <cuda_runtime.h>
 
 #include "dirac.h"
@@ -390,66 +391,65 @@ namespace b200
         int *timeout_flag;
       };
 
-      // per-stream reduction workspace
+      // Derive CG's scalars from the global sums in S[S_RAW0..]: on the device in the last block of a reduction, or on the
+      // host after the host all-reduce (no NVLink mailboxes).
+      //   FIN_PAP  v = <p, Ap>    pAp <- v, alpha = r2 / v
+      //   FIN_R2   v = |r|^2      r2_old <- r2, r2 <- v, beta = v / r2_old
+      __host__ __device__ inline void cg_scalars(double *S, int fin)
+      {
+        const double v0 = S[S_RAW0];
+        if (fin == FIN_PAP) {
+          S[S_PAP] = v0;
+          S[S_ALPHA] = S[S_R2] / v0;
+        } else if (fin == FIN_R2) {
+          const double old = S[S_R2];
+          S[S_R2_OLD] = old;
+          S[S_R2] = v0;
+          S[S_BETA] = v0 / old;
+        }
+      }
+      // A solver's scalar block: sums per reduction (kVals), block size (kCount), where the raw sums go (kRaw), and the
+      // function that derives the scalars from them.  Finaliser 0 (FIN_RAW, BF_RAW) only stores the sums.
+      struct CgTraits {
+        static constexpr int kVals = kMaxVals, kCount = S_COUNT, kRaw = S_RAW0;
+        __host__ __device__ static void derive(double *S, int fin) { cg_scalars(S, fin); }
+      };
+
+      // per-stream reduction workspace of one solver's scalar block
       struct Workspace {
-        double *partials = nullptr; // [kBlocks][kMaxVals]
+        double *partials = nullptr; // [kBlocks][kVals]
         unsigned *ticket = nullptr;
-        double *scalars = nullptr;  // [S_COUNT] on the device
-        double *host = nullptr;     // pinned + mapped: [ring][S_COUNT], written by the finalisers
+        double *scalars = nullptr;  // [kCount] on the device
+        double *host = nullptr;     // pinned + mapped: [ring][kCount], written by the finalisers
         double *host_dev = nullptr; // device alias of `host`
         cudaEvent_t ev[8] = {};
         unsigned long long ring = 0;
       };
-      // CG's workspace (partials of kMaxVals per block, S_COUNT scalars) or BiCGStab's (4 per block, its own scalars)
-      static Workspace &workspace_of(std::map<void *, Workspace> &m, void *stream, int vals, int count)
+      template <typename Tr> static Workspace &workspace(void *stream)
       {
+        static std::map<void *, Workspace> m;
         Workspace &w = m[stream];
         if (!w.partials) {
-          cuda_ok(cudaMalloc(&w.partials, sizeof(double) * kBlocks * vals), "cudaMalloc(reduce)");
+          cuda_ok(cudaMalloc(&w.partials, sizeof(double) * kBlocks * Tr::kVals), "cudaMalloc(reduce)");
           cuda_ok(cudaMalloc(&w.ticket, sizeof(unsigned)), "cudaMalloc(reduce)");
           cuda_ok(cudaMemset(w.ticket, 0, sizeof(unsigned)), "memset");
-          cuda_ok(cudaMalloc(&w.scalars, sizeof(double) * count), "cudaMalloc(reduce)");
-          cuda_ok(cudaMemset(w.scalars, 0, sizeof(double) * count), "memset");
-          cuda_ok(cudaHostAlloc(&w.host, sizeof(double) * 8 * count, cudaHostAllocMapped), "cudaHostAlloc(reduce)");
+          cuda_ok(cudaMalloc(&w.scalars, sizeof(double) * Tr::kCount), "cudaMalloc(reduce)");
+          cuda_ok(cudaMemset(w.scalars, 0, sizeof(double) * Tr::kCount), "memset");
+          cuda_ok(cudaHostAlloc(&w.host, sizeof(double) * 8 * Tr::kCount, cudaHostAllocMapped), "cudaHostAlloc(reduce)");
           cuda_ok(cudaHostGetDevicePointer(&w.host_dev, w.host, 0), "cudaHostGetDevicePointer");
           for (auto &e : w.ev) cuda_ok(cudaEventCreateWithFlags(&e, cudaEventDisableTiming), "event");
         }
         return w;
       }
-      static Workspace &workspace(void *stream)
-      {
-        static std::map<void *, Workspace> m;
-        return workspace_of(m, stream, kMaxVals, S_COUNT);
-      }
-
-      // CG's finaliser: derives pAp / alpha or r2 / beta from the global sums v[0..NV) of one reduction
-      struct CgFinish {
-        static constexpr int kVals = kMaxVals, kCount = S_COUNT;
-        template <int NV> __device__ static void apply(double *S, const double *v, int fin)
-        {
-          const double v0 = v[0];
-          if (fin == FIN_PAP) {
-            S[S_PAP] = v0;
-            S[S_ALPHA] = S[S_R2] / v0;
-          } else if (fin == FIN_R2) {
-            const double old = S[S_R2];
-            S[S_R2_OLD] = old;
-            S[S_R2] = v0;
-            S[S_BETA] = v0 / old;
-          }
-          S[S_RAW0] = v0;
-          if (NV > 1) S[S_RAW1] = v[1];
-        }
-      };
 
       // Second stage of every reduction, run by the block that arrives last: sum the per-block partial sums in block
-      // order (fixed -> bit-reproducible), all-reduce over the ranks through the NVLink mailboxes in rank order, derive
-      // the solver's scalars (Fin: CgFinish or BicgFinish) and publish the scalar block to the host mirror.
-      template <int NV, typename Fin = CgFinish>
+      // order (fixed -> bit-reproducible), all-reduce over the ranks through the NVLink mailboxes in rank order, store the
+      // global sums in the raw slots, derive the solver's scalars and publish the scalar block to the host mirror.
+      template <int NV, typename Tr>
       __device__ void finish_reduction(const double *acc_block, double *partials, unsigned *ticket, double *S, double *host_out,
                                        int fin, ReducePeers peers)
       {
-        constexpr int MV = Fin::kVals;
+        constexpr int MV = Tr::kVals;
         __shared__ double sh[kThreads][MV];
         __shared__ bool is_last;
         __shared__ double part[B200_MAX_RANKS][MV];
@@ -502,9 +502,10 @@ namespace b200
             }
         }
         if (t == 0) {
-          Fin::template apply<NV>(S, sh[0], fin);
+          for (int i = 0; i < NV; i++) S[Tr::kRaw + i] = sh[0][i];
+          Tr::derive(S, fin);
           if (host_out) {
-            for (int i = 0; i < Fin::kCount; i++) host_out[i] = S[i];
+            for (int i = 0; i < Tr::kCount; i++) host_out[i] = S[i];
             __threadfence_system();
           }
           *ticket = 0;
@@ -557,7 +558,7 @@ namespace b200
         if (R != R_NONE) {
           __shared__ double wb[kThreads / 32];
           const double s = block_sum(acc, wb);
-          finish_reduction<1>(&s, ra.partials, ra.ticket, ra.S, ra.host_out, ra.fin, ra.peers);
+          finish_reduction<1, CgTraits>(&s, ra.partials, ra.ticket, ra.S, ra.host_out, ra.fin, ra.peers);
         }
       }
 
@@ -575,7 +576,7 @@ namespace b200
         }
         __shared__ double wb[kThreads / 32];
         const double s = block_sum(acc, wb);
-        finish_reduction<1>(&s, ra.partials, ra.ticket, ra.S, ra.host_out, ra.fin, ra.peers);
+        finish_reduction<1, CgTraits>(&s, ra.partials, ra.ticket, ra.S, ra.host_out, ra.fin, ra.peers);
       }
       // x += alpha p ; p = r + beta p   (the reference's axpyZpbx, lib/inv_cg_quda.cpp:389)
       template <typename T>
@@ -609,7 +610,7 @@ namespace b200
         B_RAW = 12,   // the global sums of the last reduction, up to 4
         B_COUNT = 16
       };
-      enum BicgFinish { BF_RAW = 0, BF_RHO = 1, BF_ALPHA = 2, BF_OMEGA = 3, BF_BETA = 4 };
+      enum BicgFinish { BF_RAW = FIN_RAW, BF_RHO = 1, BF_ALPHA = 2, BF_OMEGA = 3, BF_BETA = 4 };
       enum { BRK_ALPHA = 1, BRK_OMEGA = 2, BRK_BETA = 4 };
 
       // rounded products: no FMA contraction, so that (a + ib) / (a + ib) is exactly 1 on the device and on the host
@@ -681,22 +682,12 @@ namespace b200
           if (v[2] <= S[B_STOP]) S[B_DONE] = 1.0;
         }
       }
-      struct BicgFinishOp {
-        static constexpr int kVals = 4, kCount = B_COUNT;
-        template <int NV> __device__ static void apply(double *S, const double *v, int fin)
-        {
-          for (int i = 0; i < NV; i++) S[B_RAW + i] = v[i];
-          bicg_scalars(S, fin);
-        }
+      struct BicgTraits {
+        static constexpr int kVals = 4, kCount = B_COUNT, kRaw = B_RAW;
+        __host__ __device__ static void derive(double *S, int fin) { bicg_scalars(S, fin); }
       };
 
-      template <typename T> struct Cplx;
-      template <> struct Cplx<double> {
-        using type = double2;
-      };
-      template <> struct Cplx<float> {
-        using type = float2;
-      };
+      template <typename T> using Cplx = std::conditional_t<std::is_same<T, double>::value, double2, float2>;
 
       // The five streaming kernels of a BiCGStab iteration walk the field as complex numbers: in both native orders (fp64
       // planes of 2 reals, fp32 planes of 4) the real index 2c + re/im keeps each pair adjacent, so element pair i is one
@@ -707,14 +698,14 @@ namespace b200
         double s[NV];
 #pragma unroll
         for (int i = 0; i < NV; i++) s[i] = block_sum(acc[i], wb);
-        finish_reduction<NV, BicgFinishOp>(s, ra.partials, ra.ticket, ra.S, ra.host_out, ra.fin, ra.peers);
+        finish_reduction<NV, BicgTraits>(s, ra.partials, ra.ticket, ra.S, ra.host_out, ra.fin, ra.peers);
       }
 
       // K1 (and the rho (re)computation): <a, b> = sum conj(a) b
       template <typename T>
       __global__ void __launch_bounds__(kThreads) bicg_cdot_kernel(const T *__restrict__ a_, const T *__restrict__ b_, size_t n, ReduceArgs ra)
       {
-        using C2 = typename Cplx<T>::type;
+        using C2 = Cplx<T>;
         if (ra.S[B_DONE] != 0.0) return;
         const C2 *a = reinterpret_cast<const C2 *>(a_), *b = reinterpret_cast<const C2 *>(b_);
         double acc[2] = {0, 0};
@@ -729,7 +720,7 @@ namespace b200
       template <typename T>
       __global__ void __launch_bounds__(kThreads) bicg_update_s_kernel(T *__restrict__ r_, const T *__restrict__ v_, size_t n, const double *__restrict__ S)
       {
-        using C2 = typename Cplx<T>::type;
+        using C2 = Cplx<T>;
         if (S[B_DONE] != 0.0) return;
         const double ar = S[B_ALPHA], ai = S[B_ALPHA + 1];
         C2 *r = reinterpret_cast<C2 *>(r_);
@@ -746,7 +737,7 @@ namespace b200
       template <typename T>
       __global__ void __launch_bounds__(kThreads) bicg_ts_kernel(const T *__restrict__ t_, const T *__restrict__ s_, size_t n, ReduceArgs ra)
       {
-        using C2 = typename Cplx<T>::type;
+        using C2 = Cplx<T>;
         if (ra.S[B_DONE] != 0.0) return;
         const C2 *t = reinterpret_cast<const C2 *>(t_), *s = reinterpret_cast<const C2 *>(s_);
         double acc[4] = {0, 0, 0, 0};
@@ -764,7 +755,7 @@ namespace b200
       __global__ void __launch_bounds__(kThreads) bicg_update_xr_kernel(T *__restrict__ x_, T *__restrict__ r_, const T *__restrict__ p_,
                                                                         const T *__restrict__ t_, const T *__restrict__ r0_, size_t n, ReduceArgs ra)
       {
-        using C2 = typename Cplx<T>::type;
+        using C2 = Cplx<T>;
         const double *S = ra.S;
         if (S[B_DONE] != 0.0) return;
         const double ar = S[B_ALPHA], ai = S[B_ALPHA + 1], wr = S[B_OMEGA], wi = S[B_OMEGA + 1];
@@ -791,7 +782,7 @@ namespace b200
       __global__ void __launch_bounds__(kThreads) bicg_update_p_kernel(T *__restrict__ p_, const T *__restrict__ r_, const T *__restrict__ v_,
                                                                        size_t n, const double *__restrict__ S)
       {
-        using C2 = typename Cplx<T>::type;
+        using C2 = Cplx<T>;
         if (S[B_DONE] != 0.0) return;
         const double br = S[B_BETA], bi = S[B_BETA + 1], wr = S[B_OMEGA], wi = S[B_OMEGA + 1];
         C2 *p = reinterpret_cast<C2 *>(p_);
@@ -805,18 +796,36 @@ namespace b200
           p[i] = o;
         }
       }
-      struct BicgScalars {
-        double s[B_COUNT];
+      template <int N> struct Scalars {
+        double s[N];
       };
-      __global__ void set_bicg_scalars_kernel(double *S, BicgScalars v)
+      // the whole scalar block of a solver (N <= 32)
+      template <int N> __global__ void set_scalars_kernel(double *S, Scalars<N> v)
       {
-        if (threadIdx.x < B_COUNT) S[threadIdx.x] = v.s[threadIdx.x];
+        if (threadIdx.x < N) S[threadIdx.x] = v.s[threadIdx.x];
       }
 
       static void check_pair(const ColorSpinorField &x, const ColorSpinorField &y)
       {
         if (x.Length() != y.Length()) throw Error("blas: operands differ in length");
         if (x.precision == B200_HALF || y.precision == B200_HALF) throw Error("blas: half-precision (block-float) fields are not supported");
+      }
+      template <typename... F> static void check_same(const ColorSpinorField &x, const F &...ys)
+      {
+        for (const ColorSpinorField *y : {&ys...}) {
+          check_pair(x, *y);
+          if (x.precision != y->precision) throw Error("blas: operands differ in precision (convert with blas::copy)");
+        }
+      }
+
+      // Calls f(T()) with T = double for fp64 fields and float for fp32 ones (f launches the kernel instantiated for T),
+      // then checks the launch and counts its flops.
+      template <typename F> static void launch(int precision, long long flops, F &&f)
+      {
+        if (precision == 8) f(double());
+        else f(float());
+        cuda_ok(cudaGetLastError(), "blas launch");
+        g_flops += flops;
       }
 
       static ReducePeers peers_of(CommContext *comm)
@@ -834,59 +843,70 @@ namespace b200
         }
         return p;
       }
+      static bool host_allreduce(const Exec &ex) { return ex.comm && !ex.comm->mailboxes() && ex.comm->allreduce_sum; }
 
-      // reduction launch bookkeeping: where the finaliser writes, and the event the host may wait on
+      // a reduction launched earlier: the mirror slot its finaliser writes and the event the host may wait on
       struct Pending {
         Workspace *w;
         int slot;
       };
-      static ReduceArgs reduce_args(const Exec &ex, Workspace &w, int count, int fin, Pending &pend)
-      {
-        pend.w = &w;
-        pend.slot = (int)(w.ring++ & 7);
-        ReduceArgs ra;
-        ra.partials = w.partials;
-        ra.ticket = w.ticket;
-        ra.S = w.scalars;
-        ra.host_out = w.host_dev + pend.slot * count;
-        ra.fin = fin;
-        ra.peers = peers_of(ex.comm);
-        return ra;
-      }
-      static ReduceArgs reduce_args(const Exec &ex, int fin, Pending &pend) { return reduce_args(ex, workspace(ex.stream), S_COUNT, fin, pend); }
-      static void mark(const Exec &ex, const Pending &p) { cuda_ok(cudaEventRecord(p.w->ev[p.slot], cs(ex.stream)), "record"); }
-      // wait for a reduction launched earlier and return the host mirror of the device scalars as of that launch;
-      // multi-rank sums without NVLink mailboxes go through the host callback here
-      static const double *await(const Exec &ex, const Pending &p, bool need_host_allreduce, double *scratch)
+      // wait for a reduction and return the host mirror of the solver's scalar block as of that reduction
+      template <typename Tr> static const double *await(const Pending &p)
       {
         cuda_ok(cudaEventSynchronize(p.w->ev[p.slot]), "event sync");
-        const double *h = p.w->host + p.slot * S_COUNT;
-        if (!need_host_allreduce) return h;
-        memcpy(scratch, h, sizeof(double) * S_COUNT);
-        ex.comm->allreduce_sum(&scratch[S_RAW0], 1, ex.comm->user);
-        return scratch;
+        return p.w->host + p.slot * Tr::kCount;
       }
-      static bool host_allreduce(const Exec &ex) { return ex.comm && !ex.comm->mailboxes() && ex.comm->allreduce_sum; }
+      template <typename Tr> static void set_scalar(const Exec &ex, int idx, double v)
+      {
+        set_scalar_kernel<<<1, 1, 0, cs(ex.stream)>>>(workspace<Tr>(ex.stream).scalars, idx, v);
+        cuda_ok(cudaGetLastError(), "scalar launch");
+      }
+      template <typename Tr> static void set_all(const Exec &ex, const Scalars<Tr::kCount> &s)
+      {
+        set_scalars_kernel<Tr::kCount><<<1, 32, 0, cs(ex.stream)>>>(workspace<Tr>(ex.stream).scalars, s);
+        cuda_ok(cudaGetLastError(), "scalar launch");
+      }
+      // Launch one reduction of nv sums with finaliser fin into the scalar block of Tr (kernel(T(), ra) launches it).
+      // With NVLink mailboxes, or on one rank, the last block derives the scalars on the device and nothing waits.  With
+      // the host all-reduce the kernel only stores its local sums; all nv of them go through the callback, the host
+      // derives the scalars with the same function, writes the whole block back to the device and into the mirror slot,
+      // so await() reads the same thing in both cases.  Counts the host wait in `syncs`.
+      template <typename Tr, typename K>
+      static Pending reduce(const Exec &ex, int nv, int fin, int &syncs, int precision, long long flops, K &&kernel)
+      {
+        const bool host_ar = host_allreduce(ex);
+        Workspace &w = workspace<Tr>(ex.stream);
+        const Pending pend {&w, (int)(w.ring++ & 7)};
+        const ReduceArgs ra {w.partials, w.ticket, w.scalars, w.host_dev + pend.slot * Tr::kCount, host_ar ? (int)FIN_RAW : fin,
+                             peers_of(ex.comm)};
+        launch(precision, flops, [&](auto t) { kernel(t, ra); });
+        cuda_ok(cudaEventRecord(w.ev[pend.slot], cs(ex.stream)), "record");
+        if (host_ar) {
+          Scalars<Tr::kCount> s;
+          memcpy(s.s, await<Tr>(pend), sizeof(s.s));
+          syncs++;
+          ex.comm->allreduce_sum(s.s + Tr::kRaw, nv, ex.comm->user);
+          Tr::derive(s.s, fin);
+          set_all<Tr>(ex, s);
+          memcpy(w.host + pend.slot * Tr::kCount, s.s, sizeof(s.s));
+        }
+        return pend;
+      }
 
       template <int R> static double run(double a, const ColorSpinorField &x, double b, ColorSpinorField &y, bool write, const Exec &ex)
       {
-        check_pair(x, y);
-        if (x.precision != y.precision) throw Error("blas: operands differ in precision (convert with blas::copy)");
+        check_same(x, y);
         const size_t n = x.Length();
-        Pending pend {};
-        ReduceArgs ra {};
-        if (R != R_NONE) ra = reduce_args(ex, FIN_RAW, pend);
-        cudaStream_t s = cs(ex.stream);
-        if (x.precision == 8)
-          axpby_kernel<double, double, R><<<kBlocks, kThreads, 0, s>>>(a, (const double *)x.v, b, (double *)y.v, n, write, ra);
-        else
-          axpby_kernel<float, float, R><<<kBlocks, kThreads, 0, s>>>(a, (const float *)x.v, b, (float *)y.v, n, write, ra);
-        cuda_ok(cudaGetLastError(), "blas launch");
-        g_flops += 3 * (long long)n;
-        if (R == R_NONE) return 0.0;
-        mark(ex, pend);
-        double scratch[S_COUNT];
-        return await(ex, pend, host_allreduce(ex), scratch)[S_RAW0];
+        auto axpby = [&](auto t, const ReduceArgs &ra) {
+          using T = decltype(t);
+          axpby_kernel<T, T, R><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(a, x.data<T>(), b, y.data<T>(), n, write, ra);
+        };
+        if (R == R_NONE) {
+          launch(x.precision, 3 * (long long)n, [&](auto t) { axpby(t, ReduceArgs {}); });
+          return 0.0;
+        }
+        int syncs = 0; // the callers count the wait below
+        return await<CgTraits>(reduce<CgTraits>(ex, 1, FIN_RAW, syncs, x.precision, 3 * (long long)n, axpby))[S_RAW0];
       }
 
       // Precision conversion has to go through the site/component map: the native order of fp64 fields is planes of 2
@@ -918,210 +938,114 @@ namespace b200
         const int vcb = src.VolumeCB();
         dim3 grid((vcb + 127) / 128, src.n_parity);
         const size_t se = (size_t)24 * vcb, de = (size_t)24 * vcb;
-        if (src.precision == 8)
-          convert_kernel<double, 2, float, 4><<<grid, 128, 0, cs(ex.stream)>>>((const double *)src.v, (float *)dst.v, vcb, se, de);
-        else
-          convert_kernel<float, 4, double, 2><<<grid, 128, 0, cs(ex.stream)>>>((const float *)src.v, (double *)dst.v, vcb, se, de);
-        cuda_ok(cudaGetLastError(), "convert launch");
+        launch(src.precision, 0, [&](auto t) {
+          using Ts = decltype(t);
+          using Td = std::conditional_t<sizeof(Ts) == 8, float, double>;
+          convert_kernel<Ts, 16 / sizeof(Ts), Td, 16 / sizeof(Td)><<<grid, 128, 0, cs(ex.stream)>>>(src.data<Ts>(), dst.data<Td>(), vcb, se, de);
+        });
       }
       void zero(ColorSpinorField &x, const Exec &ex) { cuda_ok(cudaMemsetAsync(x.v, 0, x.Bytes(), cs(ex.stream)), "memset"); }
-      void ax(double a, ColorSpinorField &x, const Exec &ex) { run<R_NONE>(0.0, x, a, x, true, ex); }
       void axpy(double a, const ColorSpinorField &x, ColorSpinorField &y, const Exec &ex) { run<R_NONE>(a, x, 1.0, y, true, ex); }
-      void xpay(const ColorSpinorField &x, double a, ColorSpinorField &y, const Exec &ex) { run<R_NONE>(1.0, x, a, y, true, ex); }
-      void axpby(double a, const ColorSpinorField &x, double b, ColorSpinorField &y, const Exec &ex) { run<R_NONE>(a, x, b, y, true, ex); }
       double norm2(const ColorSpinorField &x, const Exec &ex)
       {
         return run<R_NORM_Y>(0.0, x, 1.0, const_cast<ColorSpinorField &>(x), false, ex);
       }
-      double reDotProduct(const ColorSpinorField &x, const ColorSpinorField &y, const Exec &ex)
-      {
-        return run<R_DOT_XY>(0.0, x, 1.0, const_cast<ColorSpinorField &>(y), false, ex);
-      }
       double axpyNorm(double a, const ColorSpinorField &x, ColorSpinorField &y, const Exec &ex) { return run<R_NORM_Y>(a, x, 1.0, y, true, ex); }
-      double xmyNorm(const ColorSpinorField &x, ColorSpinorField &y, const Exec &ex) { return run<R_NORM_Y>(1.0, x, -1.0, y, true, ex); }
 
       // ---- CG iteration pieces (used by invertCG below)
-      static void set_scalar(const Exec &ex, int idx, double v)
-      {
-        set_scalar_kernel<<<1, 1, 0, cs(ex.stream)>>>(workspace(ex.stream).scalars, idx, v);
-        cuda_ok(cudaGetLastError(), "scalar launch");
-      }
       // <p, Ap> -> pAp, alpha = r2 / pAp (device)
-      static Pending cg_dot(const ColorSpinorField &p, const ColorSpinorField &Ap, const Exec &ex)
+      static Pending cg_dot(const ColorSpinorField &p, const ColorSpinorField &Ap, const Exec &ex, int &syncs)
       {
-        check_pair(p, Ap);
-        Pending pend {};
-        ReduceArgs ra = reduce_args(ex, FIN_PAP, pend);
+        check_same(p, Ap);
         const size_t n = p.Length();
-        if (p.precision == 8)
-          axpby_kernel<double, double, R_DOT_XY><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(0.0, (const double *)p.v, 1.0, (double *)Ap.v, n, false, ra);
-        else
-          axpby_kernel<float, float, R_DOT_XY><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(0.0, (const float *)p.v, 1.0, (float *)Ap.v, n, false, ra);
-        cuda_ok(cudaGetLastError(), "blas launch");
-        g_flops += 2 * (long long)n;
-        mark(ex, pend);
-        return pend;
+        return reduce<CgTraits>(ex, 1, FIN_PAP, syncs, p.precision, 2 * (long long)n, [&](auto t, const ReduceArgs &ra) {
+          using T = decltype(t);
+          axpby_kernel<T, T, R_DOT_XY><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(0.0, p.data<T>(), 1.0, Ap.data<T>(), n, false, ra);
+        });
       }
-      static Pending cg_update_r(ColorSpinorField &r, const ColorSpinorField &Ap, const Exec &ex)
+      static Pending cg_update_r(ColorSpinorField &r, const ColorSpinorField &Ap, const Exec &ex, int &syncs)
       {
-        check_pair(r, Ap);
-        Pending pend {};
-        ReduceArgs ra = reduce_args(ex, FIN_R2, pend);
+        check_same(r, Ap);
         const size_t n = r.Length();
-        if (r.precision == 8)
-          cg_update_r_kernel<double><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((double *)r.v, (const double *)Ap.v, n, ra);
-        else
-          cg_update_r_kernel<float><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((float *)r.v, (const float *)Ap.v, n, ra);
-        cuda_ok(cudaGetLastError(), "blas launch");
-        g_flops += 4 * (long long)n;
-        mark(ex, pend);
-        return pend;
+        return reduce<CgTraits>(ex, 1, FIN_R2, syncs, r.precision, 4 * (long long)n, [&](auto t, const ReduceArgs &ra) {
+          using T = decltype(t);
+          cg_update_r_kernel<T><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(r.data<T>(), Ap.data<T>(), n, ra);
+        });
       }
       static void cg_update_xp(ColorSpinorField &x, ColorSpinorField &p, const ColorSpinorField &r, const Exec &ex)
       {
-        check_pair(x, p);
+        check_same(x, p);
         const size_t n = p.Length();
-        const double *S = workspace(ex.stream).scalars;
-        if (p.precision == 8)
-          cg_update_xp_kernel<double><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((double *)x.v, (double *)p.v, (const double *)r.v, n, S);
-        else
-          cg_update_xp_kernel<float><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((float *)x.v, (float *)p.v, (const float *)r.v, n, S);
-        cuda_ok(cudaGetLastError(), "blas launch");
-        g_flops += 4 * (long long)n;
+        const double *S = workspace<CgTraits>(ex.stream).scalars;
+        launch(p.precision, 4 * (long long)n, [&](auto t) {
+          using T = decltype(t);
+          cg_update_xp_kernel<T><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(x.data<T>(), p.data<T>(), r.data<T>(), n, S);
+        });
       }
       static void cg_replace_r(ColorSpinorField &p, ColorSpinorField &r, const ColorSpinorField &r_new, const Exec &ex)
       {
-        check_pair(p, r_new);
+        check_same(p, r_new);
         const size_t n = p.Length();
-        if (p.precision == 8)
-          cg_replace_r_kernel<double><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((double *)p.v, (double *)r.v, (const double *)r_new.v, n);
-        else
-          cg_replace_r_kernel<float><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((float *)p.v, (float *)r.v, (const float *)r_new.v, n);
-        cuda_ok(cudaGetLastError(), "blas launch");
-        g_flops += 2 * (long long)n;
+        launch(p.precision, 2 * (long long)n, [&](auto t) {
+          using T = decltype(t);
+          cg_replace_r_kernel<T><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(p.data<T>(), r.data<T>(), r_new.data<T>(), n);
+        });
       }
 
       // ---- BiCGStab iteration pieces (used by invertBiCGStab below); all operands share the sloppy precision
-      static Workspace &bicg_workspace(void *stream)
-      {
-        static std::map<void *, Workspace> m;
-        return workspace_of(m, stream, BicgFinishOp::kVals, B_COUNT);
-      }
-      // host mirror of BiCGStab's scalar block as of a reduction launched earlier (waits for it)
-      static const double *bicg_await(const Pending &p)
-      {
-        cuda_ok(cudaEventSynchronize(p.w->ev[p.slot]), "event sync");
-        return p.w->host + p.slot * B_COUNT;
-      }
-      static void bicg_set(const Exec &ex, int idx, double v)
-      {
-        set_scalar_kernel<<<1, 1, 0, cs(ex.stream)>>>(bicg_workspace(ex.stream).scalars, idx, v);
-        cuda_ok(cudaGetLastError(), "scalar launch");
-      }
-      static void bicg_set_all(const Exec &ex, const BicgScalars &s)
-      {
-        set_bicg_scalars_kernel<<<1, 32, 0, cs(ex.stream)>>>(bicg_workspace(ex.stream).scalars, s);
-        cuda_ok(cudaGetLastError(), "scalar launch");
-      }
-      static void bicg_check(const ColorSpinorField &a, const ColorSpinorField &b)
-      {
-        check_pair(a, b);
-        if (a.precision != b.precision) throw Error("blas: operands differ in precision");
-      }
-      // Launch one BiCGStab reduction of nv sums with finaliser fin.  With NVLink mailboxes, or on one rank, the last block
-      // derives the scalars on the device and nothing waits.  With the host all-reduce the kernel only publishes its local
-      // sums; all nv of them go through the callback, the host derives the scalars with the same code, writes the whole
-      // block back to the device and into the mirror slot, so bicg_await() reads the same thing in both cases.
-      template <typename Launch>
-      static Pending bicg_reduce(const Exec &ex, int nv, int fin, bool host_ar, int &syncs, Launch &&launch)
-      {
-        Pending pend {};
-        const ReduceArgs ra = reduce_args(ex, bicg_workspace(ex.stream), B_COUNT, host_ar ? (int)BF_RAW : fin, pend);
-        launch(ra);
-        cuda_ok(cudaGetLastError(), "blas launch");
-        mark(ex, pend);
-        if (host_ar) {
-          BicgScalars s;
-          memcpy(s.s, bicg_await(pend), sizeof(s.s));
-          syncs++;
-          ex.comm->allreduce_sum(s.s + B_RAW, nv, ex.comm->user);
-          bicg_scalars(s.s, fin);
-          bicg_set_all(ex, s);
-          memcpy(pend.w->host + pend.slot * B_COUNT, s.s, sizeof(s.s));
-        }
-        return pend;
-      }
       // <a, b> (K1 with BF_ALPHA; rho = <r0, r> with BF_RHO)
-      static Pending bicg_cdot(const ColorSpinorField &a, const ColorSpinorField &b, int fin, const Exec &ex, bool host_ar, int &syncs)
+      static Pending bicg_cdot(const ColorSpinorField &a, const ColorSpinorField &b, int fin, const Exec &ex, int &syncs)
       {
-        bicg_check(a, b);
+        check_same(a, b);
         const size_t n = a.Length() / 2;
-        g_flops += 8 * (long long)n;
-        return bicg_reduce(ex, 2, fin, host_ar, syncs, [&](const ReduceArgs &ra) {
-          if (a.precision == 8)
-            bicg_cdot_kernel<double><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((const double *)a.v, (const double *)b.v, n, ra);
-          else
-            bicg_cdot_kernel<float><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((const float *)a.v, (const float *)b.v, n, ra);
+        return reduce<BicgTraits>(ex, 2, fin, syncs, a.precision, 8 * (long long)n, [&](auto t, const ReduceArgs &ra) {
+          using T = decltype(t);
+          bicg_cdot_kernel<T><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(a.data<T>(), b.data<T>(), n, ra);
         });
       }
       // K2
       static void bicg_update_s(ColorSpinorField &r, const ColorSpinorField &v, const Exec &ex)
       {
-        bicg_check(r, v);
+        check_same(r, v);
         const size_t n = r.Length() / 2;
-        const double *S = bicg_workspace(ex.stream).scalars;
-        if (r.precision == 8)
-          bicg_update_s_kernel<double><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((double *)r.v, (const double *)v.v, n, S);
-        else
-          bicg_update_s_kernel<float><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((float *)r.v, (const float *)v.v, n, S);
-        cuda_ok(cudaGetLastError(), "blas launch");
-        g_flops += 8 * (long long)n;
+        const double *S = workspace<BicgTraits>(ex.stream).scalars;
+        launch(r.precision, 8 * (long long)n, [&](auto t) {
+          using T = decltype(t);
+          bicg_update_s_kernel<T><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(r.data<T>(), v.data<T>(), n, S);
+        });
       }
       // K3
-      static Pending bicg_ts(const ColorSpinorField &t, const ColorSpinorField &s, const Exec &ex, bool host_ar, int &syncs)
+      static Pending bicg_ts(const ColorSpinorField &t, const ColorSpinorField &s, const Exec &ex, int &syncs)
       {
-        bicg_check(t, s);
+        check_same(t, s);
         const size_t n = t.Length() / 2;
-        g_flops += 16 * (long long)n;
-        return bicg_reduce(ex, 4, BF_OMEGA, host_ar, syncs, [&](const ReduceArgs &ra) {
-          if (t.precision == 8)
-            bicg_ts_kernel<double><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((const double *)t.v, (const double *)s.v, n, ra);
-          else
-            bicg_ts_kernel<float><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((const float *)t.v, (const float *)s.v, n, ra);
+        return reduce<BicgTraits>(ex, 4, BF_OMEGA, syncs, t.precision, 16 * (long long)n, [&](auto z, const ReduceArgs &ra) {
+          using T = decltype(z);
+          bicg_ts_kernel<T><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(t.data<T>(), s.data<T>(), n, ra);
         });
       }
       // K4
       static Pending bicg_update_xr(ColorSpinorField &x, ColorSpinorField &r, const ColorSpinorField &p, const ColorSpinorField &t,
-                                    const ColorSpinorField &r0, const Exec &ex, bool host_ar, int &syncs)
+                                    const ColorSpinorField &r0, const Exec &ex, int &syncs)
       {
-        bicg_check(x, r);
-        bicg_check(x, p);
-        bicg_check(x, t);
-        bicg_check(x, r0);
+        check_same(x, r, p, t, r0);
         const size_t n = x.Length() / 2;
-        g_flops += 36 * (long long)n;
-        return bicg_reduce(ex, 3, BF_BETA, host_ar, syncs, [&](const ReduceArgs &ra) {
-          if (x.precision == 8)
-            bicg_update_xr_kernel<double><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(
-              (double *)x.v, (double *)r.v, (const double *)p.v, (const double *)t.v, (const double *)r0.v, n, ra);
-          else
-            bicg_update_xr_kernel<float><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(
-              (float *)x.v, (float *)r.v, (const float *)p.v, (const float *)t.v, (const float *)r0.v, n, ra);
+        return reduce<BicgTraits>(ex, 3, BF_BETA, syncs, x.precision, 36 * (long long)n, [&](auto z, const ReduceArgs &ra) {
+          using T = decltype(z);
+          bicg_update_xr_kernel<T><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(x.data<T>(), r.data<T>(), p.data<T>(), t.data<T>(),
+                                                                            r0.data<T>(), n, ra);
         });
       }
       // K5
       static void bicg_update_p(ColorSpinorField &p, const ColorSpinorField &r, const ColorSpinorField &v, const Exec &ex)
       {
-        bicg_check(p, r);
-        bicg_check(p, v);
+        check_same(p, r, v);
         const size_t n = p.Length() / 2;
-        const double *S = bicg_workspace(ex.stream).scalars;
-        if (p.precision == 8)
-          bicg_update_p_kernel<double><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((double *)p.v, (const double *)r.v, (const double *)v.v, n, S);
-        else
-          bicg_update_p_kernel<float><<<kBlocks, kThreads, 0, cs(ex.stream)>>>((float *)p.v, (const float *)r.v, (const float *)v.v, n, S);
-        cuda_ok(cudaGetLastError(), "blas launch");
-        g_flops += 16 * (long long)n;
+        const double *S = workspace<BicgTraits>(ex.stream).scalars;
+        launch(p.precision, 16 * (long long)n, [&](auto t) {
+          using T = decltype(t);
+          bicg_update_p_kernel<T><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(p.data<T>(), r.data<T>(), v.data<T>(), n, S);
+        });
       }
     } // namespace blas
 
@@ -1330,6 +1254,117 @@ namespace b200
       site(x_other, tmp, other_parity, true);
     }
 
+    // ------------------------------------------------------------------ what CG and BiCGStab share
+    // Argument checks, the precise work fields r (residual), y (accumulated solution) and tmp, the sloppy solution xS and
+    // residual rS (r itself when both operators have one precision), the true residual in the precise operator `op`
+    // (MdagM for CG, M for BiCGStab) and the statistics of SolverParam.
+    namespace
+    {
+      struct Solve {
+        using Op = void (Dirac::*)(ColorSpinorField &, const ColorSpinorField &) const;
+        const Dirac &mat, &matSloppy;
+        const Op op;
+        ColorSpinorField &x;
+        const ColorSpinorField &b;
+        const Exec ex;
+        const std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
+        const long long flops0, ds0;
+        const int sp;
+        const bool same_prec, host_ar;
+        int syncs = 0;
+        Scratch r_s, y_s, tmp_s, xS_s;
+        std::unique_ptr<Scratch> rS_s;
+        ColorSpinorField &r = r_s.f, &y = y_s.f, &tmp = tmp_s.f, &xS = xS_s.f;
+        ColorSpinorField rS;
+        double b2 = 0.0;
+
+        // checks the arguments; returns the sloppy precision
+        static int sloppy_precision(const Dirac &mat, const Dirac &matSloppy, const ColorSpinorField &x, const ColorSpinorField &b)
+        {
+          if (matSloppy.Stream() != mat.Stream()) throw Error("precise and sloppy operators must share a stream");
+          const int sp = matSloppy.Precision();
+          if (x.precision != mat.Precision() || b.precision != mat.Precision()) throw Error("x and b must have the precise operator's precision");
+          if (sp != 8 && sp != 4) throw Error("the sloppy operator must be double or single precision");
+          if (&mat != &matSloppy && sp > x.precision) throw Error("the sloppy operator is more precise than the precise one");
+          return sp;
+        }
+        Solve(const Dirac &mat_, const Dirac &matSloppy_, Op op_, ColorSpinorField &x_, const ColorSpinorField &b_) :
+          mat(mat_), matSloppy(matSloppy_), op(op_), x(x_), b(b_), ex(mat_.exec()), flops0(blas::flops()),
+          ds0(mat_.DslashApplications() + matSloppy_.DslashApplications()), sp(sloppy_precision(mat_, matSloppy_, x_, b_)),
+          same_prec(sp == x_.precision), host_ar(blas::host_allreduce(ex)), r_s(ex.stream, x.X, x.precision, x.n_parity),
+          y_s(ex.stream, x.X, x.precision, x.n_parity), tmp_s(ex.stream, x.X, x.precision, x.n_parity), xS_s(sloppy())
+        {
+          // work fields come from the per-stream scratch pool: a second solve on the same stream allocates nothing
+          if (!same_prec) rS_s.reset(new Scratch(sloppy()));
+          rS = same_prec ? r : rS_s->f;
+        }
+        Scratch sloppy() const { return Scratch(ex.stream, x.X, sp, x.n_parity); }
+
+        // b2 = |b|^2; if b == 0, x = 0 and there is nothing to solve
+        bool zero_source(SolverParam &param)
+        {
+          b2 = blas::norm2(b, ex);
+          syncs++;
+          if (b2 != 0.0) return false;
+          blas::zero(x, ex);
+          param.iter = 0;
+          param.true_res = 0.0;
+          return true;
+        }
+        // r = b - op z in the precise operator; returns |r|^2
+        double residual(const ColorSpinorField &z)
+        {
+          (mat.*op)(tmp, z);
+          blas::copy(r, b, ex);
+          const double r2 = blas::axpyNorm(-1.0, tmp, r, ex);
+          syncs++;
+          return r2;
+        }
+        // y = x, r = b - op x, rS = r, xS = 0; returns |r|^2
+        double start()
+        {
+          blas::copy(y, x, ex);
+          const double r2 = residual(x);
+          if (!same_prec) blas::copy(rS, r, ex);
+          blas::zero(xS, ex);
+          return r2;
+        }
+        // y += xS, staged through tmp when the precisions differ
+        void fold()
+        {
+          if (same_prec) {
+            blas::axpy(1.0, xS, y, ex);
+          } else {
+            blas::copy(tmp, xS, ex);
+            blas::axpy(1.0, tmp, y, ex);
+          }
+        }
+        // reliable update: fold the sloppy solution into y, xS = 0, r = b - op y; returns |r|^2
+        double reliable_update()
+        {
+          fold();
+          blas::zero(xS, ex);
+          return residual(y);
+        }
+        // x = y + xS, its true residual, and the statistics
+        void finish(SolverParam &param, int iter)
+        {
+          fold();
+          blas::copy(x, y, ex);
+          const double tr2 = residual(x);
+          cuda_ok(cudaStreamSynchronize(cs(ex.stream)), "sync");
+          if (halo_timed_out(ex.comm, ex.stream)) throw Error("a halo wait timed out during the solve: the result is not valid");
+          param.iter = iter;
+          param.true_res = std::sqrt(tr2 / b2);
+          param.host_syncs = syncs;
+          param.secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+          const long long nds = mat.DslashApplications() + matSloppy.DslashApplications() - ds0;
+          const double fl = (double)(blas::flops() - flops0) + (double)nds * 1320.0 * x.VolumeCB();
+          param.gflops = fl / param.secs * 1e-9;
+        }
+      };
+    } // namespace
+
     // ------------------------------------------------------------------ CG (normal equations) with reliable updates
     // Same recurrences and reliable-update criterion as the reference's CG (lib/inv_cg_quda.cpp:237-420), restructured so
     // that no iteration waits for the host: pAp, r2, alpha, beta live on the device (written by the reduction
@@ -1339,76 +1374,22 @@ namespace b200
     void invertCG(const Dirac &mat, const Dirac &matSloppy, ColorSpinorField &x, const ColorSpinorField &b, SolverParam &param)
     {
       using namespace blas;
-      const Exec ex = mat.exec();
-      if (matSloppy.Stream() != mat.Stream()) throw Error("precise and sloppy operators must share a stream");
-      const auto t0 = std::chrono::steady_clock::now();
-      const long long flops0 = blas::flops();
-      const long long ds0 = mat.DslashApplications() + matSloppy.DslashApplications();
-      const bool mixed = (&mat != &matSloppy);
-      const int sp = matSloppy.Precision();
-      if (x.precision != mat.Precision() || b.precision != mat.Precision()) throw Error("x and b must have the precise operator's precision");
-      if (sp != 8 && sp != 4) throw Error("the sloppy operator must be double or single precision");
-      if (mixed && sp > x.precision) throw Error("the sloppy operator is more precise than the precise one");
-      const bool host_ar = host_allreduce(ex);
-      int syncs = 0;
+      Solve s(mat, matSloppy, &Dirac::MdagM, x, b);
+      const Exec &ex = s.ex;
+      Scratch p_s = s.sloppy(), Ap_s = s.sloppy();
+      ColorSpinorField &p = p_s.f, &Ap = Ap_s.f, &rS = s.rS;
+      if (s.zero_source(param)) return;
 
-      // work fields come from the per-stream scratch pool: a second solve on the same stream allocates nothing
-      Scratch r_s(ex.stream, x.X, x.precision, x.n_parity), y_s(ex.stream, x.X, x.precision, x.n_parity),
-        tmp_s(ex.stream, x.X, x.precision, x.n_parity);
-      ColorSpinorField &r = r_s.f;     // high-precision residual
-      ColorSpinorField &y = y_s.f;     // high-precision accumulated solution
-      ColorSpinorField &tmp = tmp_s.f;
-      const bool same_prec = sp == x.precision;
-      Scratch xS_s(ex.stream, x.X, sp, x.n_parity), p_s(ex.stream, x.X, sp, x.n_parity), Ap_s(ex.stream, x.X, sp, x.n_parity);
-      std::unique_ptr<Scratch> rS_s, tS_s;
-      if (!same_prec) {
-        rS_s.reset(new Scratch(ex.stream, x.X, sp, x.n_parity));
-        tS_s.reset(new Scratch(ex.stream, x.X, sp, x.n_parity));
-      }
-      ColorSpinorField rS = same_prec ? r : rS_s->f;
-      ColorSpinorField &xS = xS_s.f, &p = p_s.f, &Ap = Ap_s.f;
-      ColorSpinorField tS = same_prec ? tmp : tS_s->f; // sloppy-precision staging
-
-      const double b2 = norm2(b, ex);
-      syncs++;
-      if (b2 == 0.0) {
-        zero(x, ex);
-        param.iter = 0;
-        param.true_res = 0.0;
-        return;
-      }
-      // r = b - A x
-      mat.MdagM(tmp, x);
-      copy(r, b, ex);
-      double r2 = axpyNorm(-1.0, tmp, r, ex);
-      syncs++;
-      copy(y, x, ex);
-      if (!same_prec) copy(rS, r, ex);
-      zero(xS, ex);
+      double r2 = s.start();
       copy(p, rS, ex);
-      set_scalar(ex, S_R2, r2);
-      const double stop = param.tol * param.tol * b2;
+      set_scalar<CgTraits>(ex, S_R2, r2);
+      const double stop = param.tol * param.tol * s.b2;
       double rNorm = std::sqrt(r2), r0Norm = rNorm, maxrx = rNorm, maxrr = rNorm;
       int k = 0;
       param.reliable_updates = 0;
       const bool verbose = getenv("B200_CG_VERBOSE") != nullptr;
-      if (verbose) fprintf(stderr, "[cg] b2=%g r2=%g stop=%g mixed=%d\n", b2, r2, stop, (int)mixed);
+      if (verbose) fprintf(stderr, "[cg] b2=%g r2=%g stop=%g mixed=%d\n", s.b2, r2, stop, (int)(&mat != &matSloppy));
 
-      // fold the sloppy solution into y, recompute the true residual in high precision, repair the recursion
-      auto reliable_update = [&]() {
-        copy(tmp, xS, ex);
-        axpy(1.0, tmp, y, ex);
-        zero(xS, ex);
-        mat.MdagM(tmp, y);
-        copy(r, b, ex);
-        const double r2_true = axpyNorm(-1.0, tmp, r, ex);
-        syncs++;
-        copy(tS, r, ex);             // the true residual in the sloppy precision
-        cg_replace_r(p, rS, tS, ex); // p += r_true - rS ; rS = r_true
-        set_scalar(ex, S_R2, r2_true);
-        param.reliable_updates++;
-        return r2_true;
-      };
       // convergence / reliable-update decision on a residual norm; returns true if the recursion was restarted
       bool done = false;
       auto decide = [&](double r2_seen) {
@@ -1416,11 +1397,16 @@ namespace b200
         if (rNorm > maxrx) maxrx = rNorm;
         if (rNorm > maxrr) maxrr = rNorm;
         const bool converged = r2_seen <= stop;
-        const bool update = !same_prec
+        const bool update = !s.same_prec
           && ((rNorm < param.delta * maxrx && r0Norm <= maxrx) || (rNorm < param.delta * r0Norm && r0Norm <= maxrr) || converged);
         if (verbose && (k < 10 || k % 20 == 0 || update)) fprintf(stderr, "[cg] k=%d r2=%g update=%d\n", k, r2_seen, (int)update);
         if (update) {
-          r2 = reliable_update();
+          // the true residual repairs the recursion: p += r_true - rS ; rS = r_true
+          r2 = s.reliable_update();
+          copy(Ap, s.r, ex); // the true residual in the sloppy precision; Ap is free until the next iteration
+          cg_replace_r(p, rS, Ap, ex);
+          set_scalar<CgTraits>(ex, S_R2, r2);
+          param.reliable_updates++;
           rNorm = std::sqrt(r2);
           maxrr = maxrx = r0Norm = rNorm;
           if (r2 <= stop) done = true;
@@ -1432,67 +1418,27 @@ namespace b200
 
       Pending prev {};
       bool have_prev = false;
-      double scratch[S_COUNT];
       while (!done && k < param.maxiter) {
         matSloppy.MdagM(Ap, p);
-        Pending pd = cg_dot(p, Ap, ex);
-        if (host_ar) { // no NVLink mailboxes: every global sum goes through the host callback (two syncs per iteration)
-          const double pAp = await(ex, pd, true, scratch)[S_RAW0];
-          syncs++;
-          set_scalar(ex, S_PAP, pAp);
-          set_scalar(ex, S_ALPHA, r2 / pAp);
-        }
-        Pending pr = cg_update_r(rS, Ap, ex);
-        if (host_ar) {
-          const double r2_new = await(ex, pr, true, scratch)[S_RAW0];
-          syncs++;
-          set_scalar(ex, S_R2_OLD, r2);
-          set_scalar(ex, S_R2, r2_new);
-          set_scalar(ex, S_BETA, r2_new / r2);
-          r2 = r2_new;
-        }
-        cg_update_xp(xS, p, rS, ex);
+        cg_dot(p, Ap, ex, s.syncs);
+        Pending pr = cg_update_r(rS, Ap, ex, s.syncs);
+        cg_update_xp(s.xS, p, rS, ex);
         k++;
-        if (host_ar) {
-          decide(r2);
+        if (s.host_ar) { // every reduction has already been waited for
+          decide(await<CgTraits>(pr)[S_R2]);
           continue;
         }
         // the host follows one iteration behind: while the GPU runs iteration k it looks at the residual of k - 1
         bool restarted = false;
         if (have_prev) {
-          r2 = await(ex, prev, false, scratch)[S_R2];
-          syncs++;
-          restarted = decide(r2);
+          restarted = decide(await<CgTraits>(prev)[S_R2]);
+          s.syncs++;
         }
-        if (restarted) {
-          have_prev = false; // the pending residual belongs to the recursion before the restart
-        } else {
-          prev = pr;
-          have_prev = true;
-        }
+        // after a restart the pending residual belongs to the recursion before it
+        have_prev = !restarted;
+        prev = pr;
       }
-      // x = y + xS
-      if (same_prec) {
-        axpy(1.0, xS, y, ex);
-      } else {
-        copy(tmp, xS, ex);
-        axpy(1.0, tmp, y, ex);
-      }
-      copy(x, y, ex);
-      // true residual
-      mat.MdagM(tmp, x);
-      copy(r, b, ex);
-      const double tr2 = axpyNorm(-1.0, tmp, r, ex);
-      syncs++;
-      cuda_ok(cudaStreamSynchronize(cs(ex.stream)), "sync");
-      if (halo_timed_out(ex.comm, ex.stream)) throw Error("a halo wait timed out during the solve: the result is not valid");
-      param.iter = k;
-      param.true_res = std::sqrt(tr2 / b2);
-      param.host_syncs = syncs;
-      param.secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-      const long long nds = mat.DslashApplications() + matSloppy.DslashApplications() - ds0;
-      const double fl = (double)(blas::flops() - flops0) + (double)nds * 1320.0 * x.VolumeCB();
-      param.gflops = fl / param.secs * 1e-9;
+      s.finish(param, k);
     }
 
     // ------------------------------------------------------------------ BiCGStab (M x = b) with reliable updates
@@ -1510,81 +1456,37 @@ namespace b200
     void invertBiCGStab(const Dirac &mat, const Dirac &matSloppy, ColorSpinorField &x, const ColorSpinorField &b, SolverParam &param)
     {
       using namespace blas;
-      const Exec ex = mat.exec();
-      if (matSloppy.Stream() != mat.Stream()) throw Error("precise and sloppy operators must share a stream");
-      const auto t0 = std::chrono::steady_clock::now();
-      const long long flops0 = blas::flops();
-      const long long ds0 = mat.DslashApplications() + matSloppy.DslashApplications();
-      const bool mixed = (&mat != &matSloppy);
-      const int sp = matSloppy.Precision();
-      if (x.precision != mat.Precision() || b.precision != mat.Precision()) throw Error("x and b must have the precise operator's precision");
-      if (sp != 8 && sp != 4) throw Error("the sloppy operator must be double or single precision");
-      if (mixed && sp > x.precision) throw Error("the sloppy operator is more precise than the precise one");
-      const bool host_ar = host_allreduce(ex);
-      int syncs = 0;
-
-      Scratch r_s(ex.stream, x.X, x.precision, x.n_parity), y_s(ex.stream, x.X, x.precision, x.n_parity),
-        tmp_s(ex.stream, x.X, x.precision, x.n_parity);
-      ColorSpinorField &r = r_s.f;     // high-precision residual
-      ColorSpinorField &y = y_s.f;     // high-precision accumulated solution
-      ColorSpinorField &tmp = tmp_s.f;
-      const bool same_prec = sp == x.precision;
-      Scratch xS_s(ex.stream, x.X, sp, x.n_parity), p_s(ex.stream, x.X, sp, x.n_parity), v_s(ex.stream, x.X, sp, x.n_parity),
-        t_s(ex.stream, x.X, sp, x.n_parity), r0_s(ex.stream, x.X, sp, x.n_parity);
-      std::unique_ptr<Scratch> rS_s;
-      if (!same_prec) rS_s.reset(new Scratch(ex.stream, x.X, sp, x.n_parity));
-      ColorSpinorField rS = same_prec ? r : rS_s->f; // sloppy residual; holds s between K2 and K4
-      ColorSpinorField &xS = xS_s.f, &p = p_s.f, &v = v_s.f, &t = t_s.f, &r0 = r0_s.f;
-
-      const double b2 = norm2(b, ex);
-      syncs++;
-      if (b2 == 0.0) {
-        zero(x, ex);
-        param.iter = 0;
-        param.true_res = 0.0;
-        return;
-      }
-      const double stop = param.tol * param.tol * b2;
+      Solve s(mat, matSloppy, &Dirac::M, x, b);
+      const Exec &ex = s.ex;
+      Scratch p_s = s.sloppy(), v_s = s.sloppy(), t_s = s.sloppy(), r0_s = s.sloppy();
+      ColorSpinorField &p = p_s.f, &v = v_s.f, &t = t_s.f, &r0 = r0_s.f;
+      ColorSpinorField &rS = s.rS; // sloppy residual; holds s between K2 and K4
+      if (s.zero_source(param)) return;
+      const double stop = param.tol * param.tol * s.b2;
       double r2 = 0.0, maxrr = 0.0;
       int k = 0;
       param.reliable_updates = 0;
 
-      // y += x_sloppy, r = b - M y in the precise operator, r_sloppy = r; clears the device flags
+      // reliable update in the precise operator, then rS = r; clears the device flags
       auto true_residual = [&]() {
-        if (same_prec) {
-          axpy(1.0, xS, y, ex);
-        } else {
-          copy(tmp, xS, ex);
-          axpy(1.0, tmp, y, ex);
-        }
-        zero(xS, ex);
-        mat.M(tmp, y);
-        copy(r, b, ex);
-        r2 = axpyNorm(-1.0, tmp, r, ex);
-        syncs++;
-        if (!same_prec) copy(rS, r, ex);
-        bicg_set(ex, B_R2, r2);
-        bicg_set(ex, B_DONE, 0.0);
-        bicg_set(ex, B_BREAK, 0.0);
+        r2 = s.reliable_update();
+        if (!s.same_prec) copy(rS, s.r, ex);
+        set_scalar<BicgTraits>(ex, B_R2, r2);
+        set_scalar<BicgTraits>(ex, B_DONE, 0.0);
+        set_scalar<BicgTraits>(ex, B_BREAK, 0.0);
         maxrr = std::sqrt(r2);
       };
-      auto recompute_rho = [&]() { bicg_cdot(r0, rS, BF_RHO, ex, host_ar, syncs); };
+      auto recompute_rho = [&]() { bicg_cdot(r0, rS, BF_RHO, ex, s.syncs); };
 
       // r = b - M x, r0 = p = r, rho = <r0, r>
-      copy(y, x, ex);
-      mat.M(tmp, x);
-      copy(r, b, ex);
-      r2 = axpyNorm(-1.0, tmp, r, ex);
-      syncs++;
+      r2 = s.start();
       maxrr = std::sqrt(r2);
-      if (!same_prec) copy(rS, r, ex);
-      zero(xS, ex);
       copy(r0, rS, ex);
       copy(p, rS, ex);
-      BicgScalars s0 {};
+      Scalars<B_COUNT> s0 {};
       s0.s[B_R2] = r2;
       s0.s[B_STOP] = stop;
-      bicg_set_all(ex, s0);
+      set_all<BicgTraits>(ex, s0);
       recompute_rho();
       bool done = r2 <= stop;
 
@@ -1599,7 +1501,7 @@ namespace b200
           true_residual();
           copy(r0, rS, ex);
           copy(p, rS, ex);
-        } else if (!same_prec && (converged || rNorm < param.delta * maxrr)) {
+        } else if (!s.same_prec && (converged || rNorm < param.delta * maxrr)) {
           true_residual(); // reliable update: p is kept
         } else {
           done = converged;
@@ -1615,48 +1517,29 @@ namespace b200
       bool have_prev = false;
       while (!done && k < param.maxiter) {
         matSloppy.M(v, p);
-        bicg_cdot(r0, v, BF_ALPHA, ex, host_ar, syncs);    // K1
-        bicg_update_s(rS, v, ex);                           // K2
+        bicg_cdot(r0, v, BF_ALPHA, ex, s.syncs);                      // K1
+        bicg_update_s(rS, v, ex);                                      // K2
         matSloppy.M(t, rS);
-        bicg_ts(t, rS, ex, host_ar, syncs);                 // K3
-        Pending p4 = bicg_update_xr(xS, rS, p, t, r0, ex, host_ar, syncs); // K4
-        bicg_update_p(p, rS, v, ex);                        // K5
+        bicg_ts(t, rS, ex, s.syncs);                                   // K3
+        Pending p4 = bicg_update_xr(s.xS, rS, p, t, r0, ex, s.syncs); // K4
+        bicg_update_p(p, rS, v, ex);                                   // K5
         k++;
-        if (host_ar) { // every reduction has already been waited for
-          decide(bicg_await(p4), k);
+        if (s.host_ar) { // every reduction has already been waited for
+          decide(await<BicgTraits>(p4), k);
           continue;
         }
         bool replaced = false;
         if (have_prev) {
-          replaced = decide(bicg_await(prev), k - 1);
-          syncs++;
+          replaced = decide(await<BicgTraits>(prev), k - 1);
+          s.syncs++;
         }
         // after a replacement the pending scalars belong to the recursion before it
         have_prev = !replaced;
         prev = p4;
       }
-      // x = y + x_sloppy
-      if (same_prec) {
-        axpy(1.0, xS, y, ex);
-      } else {
-        copy(tmp, xS, ex);
-        axpy(1.0, tmp, y, ex);
-      }
-      copy(x, y, ex);
-      mat.M(tmp, x);
-      copy(r, b, ex);
-      const double tr2 = axpyNorm(-1.0, tmp, r, ex);
-      syncs++;
-      cuda_ok(cudaStreamSynchronize(cs(ex.stream)), "sync");
-      if (halo_timed_out(ex.comm, ex.stream)) throw Error("a halo wait timed out during the solve: the result is not valid");
-      param.iter = k;
-      param.true_res = std::sqrt(tr2 / b2);
-      param.host_syncs = syncs;
-      param.secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-      const long long nds = mat.DslashApplications() + matSloppy.DslashApplications() - ds0;
-      const double fl = (double)(blas::flops() - flops0) + (double)nds * 1320.0 * x.VolumeCB();
-      param.gflops = fl / param.secs * 1e-9;
+      s.finish(param, k);
     }
 
   } // namespace host
 } // namespace b200
+

@@ -18,7 +18,7 @@ struct b200_dirac_s {
   bool has_clover = false;
   CommContext comm;
   bool has_comm = false;
-  b200_comm *user_comm = nullptr; // seq is mirrored back so that all layers agree on the buffer parity
+  b200_comm *user_comm = nullptr; // the caller's exchange: pull_comm mirrors it into `comm` before every call
   int precision = 0;
   int X[4];
   std::unique_ptr<Dirac> op;
@@ -49,7 +49,6 @@ static void pull_comm(b200_dirac_s *h)
   memcpy(k.reduce_peer, c->reduce_peer, sizeof(k.reduce_peer));
   k.reduce_seq_shared = &c->reduce_seq;
 }
-static void push_comm(b200_dirac_s *) { }
 
 template <typename F> static int guarded(F &&f)
 {
@@ -143,16 +142,14 @@ int b200_dirac_apply(b200_dirac *h, int what, const b200_spinor *out, const b200
       }
     } catch (...) {
       if (dagger) h->op->flipDagger();
-      push_comm(h);
       throw;
     }
     if (dagger) h->op->flipDagger();
-    push_comm(h);
   });
 }
 
 /* 0 if no halo wait has given up since the last check on this exchange; B200_ERR_CUDA (and the flag is cleared) otherwise.
- * Synchronises `stream`.  b200_invert_cg checks by itself; callers of b200_dirac_apply / b200_dslash_apply on partitioned
+ * Synchronises `stream`.  The solvers check by themselves; callers of b200_dirac_apply / b200_dslash_apply on partitioned
  * lattices call this at their own synchronisation points. */
 int b200_comm_check(b200_comm *c, void *stream)
 {
@@ -174,7 +171,6 @@ int b200_dirac_prepare(b200_dirac *h, const b200_spinor *x, const b200_spinor *b
     const size_t pb = xf.parity_bytes;
     if (src_parity) *src_parity = (int)((static_cast<char *>(src.v) - static_cast<char *>(xf.v)) / (long)pb);
     if (sol_parity) *sol_parity = (int)((static_cast<char *>(sol.v) - static_cast<char *>(xf.v)) / (long)pb);
-    push_comm(h);
   });
 }
 
@@ -184,52 +180,48 @@ int b200_dirac_reconstruct(b200_dirac *h, const b200_spinor *x, const b200_spino
     pull_comm(h);
     auto xf = wrap(h, x), bf = wrap(h, b);
     h->op->reconstruct(xf, bf, QUDA_MAT_SOLUTION);
-    push_comm(h);
   });
 }
 
 using Solver = void (*)(const Dirac &, const Dirac &, ColorSpinorField &, const ColorSpinorField &, SolverParam &);
 
-// comm mirroring and parameter marshaling shared by the solver entry points
-static void invert(Solver solve, b200_dirac *precise, b200_dirac *sloppy, const b200_spinor *x, const b200_spinor *b,
-                   b200_solver_param *param)
+// argument checks, comm mirroring and parameter marshaling shared by the solver entry points
+static int invert(const char *name, Solver solve, b200_dirac *precise, b200_dirac *sloppy, const b200_spinor *x,
+                  const b200_spinor *b, b200_solver_param *param)
 {
-  if (!sloppy) sloppy = precise;
-  pull_comm(precise);
-  if (sloppy != precise) {
-    // a partitioned mixed-precision solve needs one halo context per precision (the ghost buffers differ in size);
-    // both advance in lock step on every rank because all ranks execute the same operator sequence
-    if (precise->has_comm != sloppy->has_comm) throw Error("precise / sloppy operators disagree on partitioning");
-    pull_comm(sloppy);
-  }
-  auto xf = wrap(precise, x), bf = wrap(precise, b);
-  SolverParam sp;
-  sp.tol = param->tol;
-  sp.maxiter = param->maxiter;
-  sp.delta = param->delta > 0 ? param->delta : 0.1;
-  solve(*precise->op, *sloppy->op, xf, bf, sp);
-  param->iter = sp.iter;
-  param->reliable_updates = sp.reliable_updates;
-  param->true_res = sp.true_res;
-  param->secs = sp.secs;
-  param->gflops = sp.gflops;
-  param->host_syncs = sp.host_syncs;
-  push_comm(precise);
-  if (sloppy != precise) push_comm(sloppy);
+  if (!precise || !param) return b200::set_error(B200_ERR_INVALID, "%s: null argument", name);
+  if (int rc = b200::require_device()) return rc;
+  return guarded([&] {
+    if (!sloppy) sloppy = precise;
+    pull_comm(precise);
+    if (sloppy != precise) {
+      // a partitioned mixed-precision solve needs one halo context per precision (the ghost buffers differ in size);
+      // both advance in lock step on every rank because all ranks execute the same operator sequence
+      if (precise->has_comm != sloppy->has_comm) throw Error("precise / sloppy operators disagree on partitioning");
+      pull_comm(sloppy);
+    }
+    auto xf = wrap(precise, x), bf = wrap(precise, b);
+    SolverParam sp;
+    sp.tol = param->tol;
+    sp.maxiter = param->maxiter;
+    sp.delta = param->delta > 0 ? param->delta : 0.1;
+    solve(*precise->op, *sloppy->op, xf, bf, sp);
+    param->iter = sp.iter;
+    param->reliable_updates = sp.reliable_updates;
+    param->true_res = sp.true_res;
+    param->secs = sp.secs;
+    param->gflops = sp.gflops;
+    param->host_syncs = sp.host_syncs;
+  });
 }
 
 int b200_invert_bicgstab(b200_dirac *precise, b200_dirac *sloppy, const b200_spinor *x, const b200_spinor *b, b200_solver_param *param)
 {
-  if (!precise || !param) return b200::set_error(B200_ERR_INVALID, "b200_invert_bicgstab: null argument");
-  if (int rc = b200::require_device()) return rc;
-  return guarded([&] { invert(invertBiCGStab, precise, sloppy, x, b, param); });
+  return invert("b200_invert_bicgstab", invertBiCGStab, precise, sloppy, x, b, param);
 }
 
 int b200_invert_cg(b200_dirac *precise, b200_dirac *sloppy, const b200_spinor *x, const b200_spinor *b, b200_solver_param *param)
 {
-  return guarded([&] {
-    if (!precise || !param) throw Error("b200_invert_cg: null argument");
-    invert(invertCG, precise, sloppy, x, b, param);
-  });
+  return invert("b200_invert_cg", invertCG, precise, sloppy, x, b, param);
 }
 }

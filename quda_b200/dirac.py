@@ -1,6 +1,7 @@
 """Thin Python handles on the C++ operator / solver layer (quda_b200/csrc/host/dirac.h): DiracWilson[PC],
-DiracClover[PC] (reference: lib/dirac_wilson.cpp, lib/dirac_clover.cpp) and CG with reliable updates
-(lib/inv_cg_quda.cpp).  All arithmetic happens in libquda_b200.so; this module only marshals descriptors."""
+DiracClover[PC], DiracTwistedMass[PC] (reference: lib/dirac_wilson.cpp, lib/dirac_clover.cpp, lib/dirac_twisted_mass.cpp),
+CG on the normal equations (lib/inv_cg_quda.cpp) and BiCGStab on M itself (lib/inv_bicgstab_quda.cpp), both mixed-precision
+with reliable updates.  All arithmetic happens in libquda_b200.so; this module only marshals descriptors."""
 import ctypes as C
 
 from . import lib as L
@@ -69,24 +70,25 @@ class Dirac:
         L.check(self.lib.b200_dirac_reconstruct(self.h, C.byref(xd), C.byref(bd)))
 
 
-def invert_cg(precise, sloppy, x, b, tol=1e-10, maxiter=10000, delta=0.1):
-    """CG on MdagM x = b; returns the filled SolverParam (iter, true_res, secs, gflops, reliable_updates)."""
+def _invert(name, precise, sloppy, x, b, tol, maxiter, delta):
+    """Run the C ABI solver b200_<name>; returns the filled SolverParam (iter, true_res, secs, gflops, reliable_updates,
+    host_syncs).  x and b must have the precise operator's precision: the C ABI reads them in that precision."""
+    for what, f in (("x", x), ("b", b)):
+        if f.prec != precise.prec:
+            raise L.B200Error(f"{name}: {what} has precision {f.prec}, the precise operator {precise.prec}")
     p = L.SolverParam()
     p.tol, p.maxiter, p.delta = tol, maxiter, delta
     xd, bd = x.desc(), b.desc()
-    L.check(precise.lib.b200_invert_cg(precise.h, sloppy.h if sloppy is not None else None, C.byref(xd), C.byref(bd), C.byref(p)))
+    solve = getattr(precise.lib, "b200_" + name)
+    L.check(solve(precise.h, sloppy.h if sloppy is not None else None, C.byref(xd), C.byref(bd), C.byref(p)))
     return p
+
+
+def invert_cg(precise, sloppy, x, b, tol=1e-10, maxiter=10000, delta=0.1):
+    """CG on MdagM x = b (lib/inv_cg_quda.cpp)."""
+    return _invert("invert_cg", precise, sloppy, x, b, tol, maxiter, delta)
 
 
 def invert_bicgstab(precise, sloppy, x, b, tol=1e-10, maxiter=10000, delta=0.1):
-    """BiCGStab on M x = b with the operator as given (lib/inv_bicgstab_quda.cpp); returns the filled SolverParam.
-    x and b must have the precise operator's precision (the C ABI reads them in that precision)."""
-    for name, f in (("x", x), ("b", b)):
-        if f.prec != precise.prec:
-            raise L.B200Error(f"invert_bicgstab: {name} has precision {f.prec}, the precise operator {precise.prec}")
-    p = L.SolverParam()
-    p.tol, p.maxiter, p.delta = tol, maxiter, delta
-    xd, bd = x.desc(), b.desc()
-    L.check(precise.lib.b200_invert_bicgstab(precise.h, sloppy.h if sloppy is not None else None, C.byref(xd), C.byref(bd),
-                                             C.byref(p)))
-    return p
+    """BiCGStab on M x = b with the operator as given (lib/inv_bicgstab_quda.cpp)."""
+    return _invert("invert_bicgstab", precise, sloppy, x, b, tol, maxiter, delta)
