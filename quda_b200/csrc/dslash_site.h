@@ -155,6 +155,9 @@ namespace b200
     return cb_from_coords(y, g);
   }
 
+  // projector sign of a hop: the forward hop uses P(d, dagger ? + : -), the backward hop P(d, dagger ? - : +)
+  template <bool dagger, bool fwd> B2_HD constexpr int hop_sign() { return fwd ? (dagger ? +1 : -1) : (dagger ? -1 : +1); }
+
   // Links whose packed form is small enough (<= 48 B: fp32 recon-12/8, every half format) are fetched for all 8 hops
   // before the first hop is computed (<= 96 registers of raw vectors): one exposed DRAM round trip per site for the
   // link stream instead of one per hop.  Wider links (fp64, fp32 recon-18) would not fit the register file.
@@ -164,6 +167,17 @@ namespace b200
   template <class P, int recon> struct PreloadLinks {
     static constexpr bool value = B2_PRELOAD_LINKS && (sizeof(typename GaugeView<P, recon>::Raw) <= 48);
   };
+
+  // the 8 packed links of site x: raw[2d] = U_d(x) (forward hop), raw[2d + 1] = U_d(x - d) (backward hop)
+  template <class P, int recon, Cache lc = Cache::STREAM>
+  B2_HD void load_links(typename GaugeView<P, recon>::Raw *raw, const DslashArgs<P, recon> &arg, const int *x, int x_cb, int parity)
+  {
+#pragma unroll
+    for (int d = 0; d < 4; d++) {
+      arg.U.template load_raw<lc>(raw[2 * d], d, x_cb, parity);
+      arg.U.template load_raw<lc>(raw[2 * d + 1], d, neighbor_cb<false>(x, arg.geom, d), 1 - parity);
+    }
+  }
 
   // v <- s (v + b i gamma5 v).  In the UKQCD basis gamma5 exchanges the spin pairs: (i gamma5 v)_s = i v_{s +- 2}
   // (include/color_spinor.h:254-262, igamma(4)).
@@ -183,25 +197,69 @@ namespace b200
     }
   }
 
-  // `in` is passed explicitly so that the multi-RHS kernels can aim the same code at any source; `lc` is the cache
-  // policy of the link loads; `pretwist`: the neighbour spinor is rotated by a (1 + i b gamma5) before it is projected
-  // (symmetric preconditioned twisted-mass dagger, applyWilsonTM)
-  template <class P, int recon, bool dagger, bool fwd, Cache lc = Cache::STREAM, bool pretwist = false>
-  B2_HD void hop_from(typename P::real *r, const DslashArgs<P, recon> &arg, const SpinorView<P> &in, const int *x, int x_cb,
-                      int parity, int d, const typename GaugeView<P, recon>::Raw *raw = nullptr)
+  // Half precision: keep the int16 values of link and neighbour spinor unscaled through projection and SU(3) multiply
+  // (exact small integers in fp32) and apply link scale x block-float norm (x 2 for the t direction) in the single
+  // FFMA per component that accumulates the hop.  Removes ~250 of the 2 400 instructions per site of the issue-bound
+  // half kernels.  B2_HALF_DEFERRED_SCALE=0 restores the scale-on-load arithmetic.
+#ifndef B2_HALF_DEFERRED_SCALE
+#define B2_HALF_DEFERRED_SCALE 1
+#endif
+  template <class P> struct DeferredScale {
+    static constexpr bool value = P::fixed && B2_HALF_DEFERRED_SCALE;
+  };
+
+  // Link part of a hop: u = U_d(x) (forward) or U_d(x - d) (backward), unpacked from the preloaded `raw` or loaded with
+  // cache policy `lc`.  With deferred scaling `u` stays unscaled and `us` is its scale.
+  template <class P, int recon, bool fwd, Cache lc>
+  B2_HD void hop_link(typename P::real *u, typename P::real &us, const DslashArgs<P, recon> &arg, int x_cb, int n_cb, int parity,
+                      int d, const typename GaugeView<P, recon>::Raw *raw)
+  {
+    if constexpr (DeferredScale<P>::value) {
+      if (raw) {
+        arg.U.unpack_deferred(u, us, *raw, d, fwd ? x_cb : n_cb);
+      } else {
+        typename GaugeView<P, recon>::Raw w;
+        arg.U.template load_raw<lc>(w, d, fwd ? x_cb : n_cb, fwd ? parity : 1 - parity);
+        arg.U.unpack_deferred(u, us, w, d, fwd ? x_cb : n_cb);
+      }
+    } else if (raw) {
+      arg.U.unpack(u, *raw, d, fwd ? x_cb : n_cb);
+    } else if (fwd) {
+      arg.U.template load<lc>(u, d, x_cb, parity);
+    } else {
+      arg.U.template load<lc>(u, d, n_cb, 1 - parity);
+    }
+  }
+
+  // Spinor part of a hop: r = (U or U^dagger) P h for the neighbour spinor h of `in` at n_cb.  With deferred scaling h
+  // and r stay unscaled and `scale` is the factor r still has to be multiplied by (link scale `us` x block-float norm).
+  // `pretwist`: the neighbour spinor is rotated by a (1 + i b gamma5) before it is projected (symmetric preconditioned
+  // twisted-mass dagger, applyWilsonTM).
+  template <class P, int recon, bool dagger, bool fwd, bool pretwist = false>
+  B2_HD void hop_spinor(typename P::real *r, typename P::real &scale, const typename P::real *u, typename P::real us,
+                        const DslashArgs<P, recon> &arg, const SpinorView<P> &in, int n_cb, int d)
   {
     using real = typename P::real;
-    const Geom &g = arg.geom;
-    constexpr int sign = fwd ? (dagger ? +1 : -1) : (dagger ? -1 : +1);
-    real u[18], h[12];
-    const int n_cb = neighbor_cb<fwd>(x, g, d);
-    if (raw)
-      arg.U.unpack(u, *raw, d, fwd ? x_cb : n_cb);
-    else if (fwd)
-      arg.U.template load<lc>(u, d, x_cb, parity);
-    else
-      arg.U.template load<lc>(u, d, n_cb, 1 - parity);
-    if constexpr (pretwist) { // gamma5 mixes the spin pairs: the full spinor is needed in every direction
+    constexpr int sign = hop_sign<dagger, fwd>();
+    real h[12];
+    if constexpr (DeferredScale<P>::value) {
+      const real n = in.load_norm(n_cb);
+      if constexpr (pretwist) { // the rotation is linear, so it commutes with the deferred scale; project() carries t's factor 2
+        real v[24];
+        in.template load_planes<0, 24 / P::Ns>(v, n_cb);
+        twist_apply(v, arg.a, arg.twist_b());
+        project(h, v, d, sign);
+        scale = us * n;
+      } else if (d == 3) {
+        load_spin_pair<P, (sign > 0), Cache::REUSE, false>(h, in, n_cb);
+        scale = (us * n) * (real)2;
+      } else {
+        real v[24];
+        in.template load_planes<0, 24 / P::Ns>(v, n_cb);
+        project(h, v, d, sign);
+        scale = us * n;
+      }
+    } else if constexpr (pretwist) { // gamma5 mixes the spin pairs: the full spinor is needed in every direction
       real v[24];
       in.load(v, n_cb);
       twist_apply(v, arg.a, arg.twist_b());
@@ -219,59 +277,24 @@ namespace b200
     su3_mul<!fwd>(r, u, h);
   }
 
-  template <class P, int recon, bool dagger, bool fwd>
-  B2_HD void hop_local(typename P::real *r, const DslashArgs<P, recon> &arg, const int *x, int x_cb, int parity, int d,
-                       const typename GaugeView<P, recon>::Raw *raw = nullptr)
+  // One local hop, link part then spinor part.  `in` is passed explicitly so that the multi-RHS kernels can aim the same
+  // code at any source; `scale` is set with deferred scaling only.
+  template <class P, int recon, bool dagger, bool fwd, Cache lc = Cache::STREAM, bool pretwist = false>
+  B2_HD void hop_from(typename P::real *r, typename P::real &scale, const DslashArgs<P, recon> &arg, const SpinorView<P> &in,
+                      const int *x, int x_cb, int parity, int d, const typename GaugeView<P, recon>::Raw *raw = nullptr)
   {
-    hop_from<P, recon, dagger, fwd>(r, arg, arg.in[1 - parity], x, x_cb, parity, d, raw);
+    typename P::real u[18], us = 1;
+    const int n_cb = neighbor_cb<fwd>(x, arg.geom, d);
+    hop_link<P, recon, fwd, lc>(u, us, arg, x_cb, n_cb, parity, d, raw);
+    hop_spinor<P, recon, dagger, fwd, pretwist>(r, scale, u, us, arg, in, n_cb, d);
   }
 
-  // Half precision: keep the int16 values of link and neighbour spinor unscaled through projection and SU(3) multiply
-  // (exact small integers in fp32) and apply link scale x block-float norm (x 2 for the t direction) in the single
-  // FFMA per component that accumulates the hop.  Removes ~250 of the 2 400 instructions per site of the issue-bound
-  // half kernels.  B2_HALF_DEFERRED_SCALE=0 restores the scale-on-load arithmetic.
-#ifndef B2_HALF_DEFERRED_SCALE
-#define B2_HALF_DEFERRED_SCALE 1
-#endif
-  template <class P> struct DeferredScale {
-    static constexpr bool value = P::fixed && B2_HALF_DEFERRED_SCALE;
-  };
-
-  // r = (U or U^dagger) P h with everything unscaled; `scale` is the factor the result still has to be multiplied by
-  template <class P, int recon, bool dagger, bool fwd, Cache lc = Cache::STREAM, bool pretwist = false>
-  B2_HD void hop_from_deferred(typename P::real *r, typename P::real &scale, const DslashArgs<P, recon> &arg,
-                               const SpinorView<P> &in, const int *x, int x_cb, int parity, int d,
-                               const typename GaugeView<P, recon>::Raw *raw = nullptr)
+  // hop_from on the launch's own input field, for callers without deferred scaling
+  template <class P, int recon, bool dagger, bool fwd>
+  B2_HD void hop_local(typename P::real *r, const DslashArgs<P, recon> &arg, const int *x, int x_cb, int parity, int d)
   {
-    using real = typename P::real;
-    const Geom &g = arg.geom;
-    constexpr int sign = fwd ? (dagger ? +1 : -1) : (dagger ? -1 : +1);
-    real u[18], h[12], us;
-    const int n_cb = neighbor_cb<fwd>(x, g, d);
-    if (raw) {
-      arg.U.unpack_deferred(u, us, *raw, d, fwd ? x_cb : n_cb);
-    } else {
-      typename GaugeView<P, recon>::Raw w;
-      arg.U.template load_raw<lc>(w, d, fwd ? x_cb : n_cb, fwd ? parity : 1 - parity);
-      arg.U.unpack_deferred(u, us, w, d, fwd ? x_cb : n_cb);
-    }
-    const real n = in.load_norm(n_cb);
-    if constexpr (pretwist) { // the rotation is linear, so it commutes with the deferred scale; project() carries t's factor 2
-      real v[24];
-      in.template load_planes<0, 24 / P::Ns>(v, n_cb);
-      twist_apply(v, arg.a, arg.twist_b());
-      project(h, v, d, sign);
-      scale = us * n;
-    } else if (d == 3) {
-      load_spin_pair<P, (sign > 0), Cache::REUSE, false>(h, in, n_cb);
-      scale = (us * n) * (real)2;
-    } else {
-      real v[24];
-      in.template load_planes<0, 24 / P::Ns>(v, n_cb);
-      project(h, v, d, sign);
-      scale = us * n;
-    }
-    su3_mul<!fwd>(r, u, h);
+    typename P::real scale;
+    hop_from<P, recon, dagger, fwd>(r, scale, arg, arg.in[1 - parity], x, x_cb, parity, d);
   }
 
   // acc += hop (+ optional 0/1 mask for the masked interior kernel); every local hop of every kernel goes through here
@@ -280,15 +303,13 @@ namespace b200
                      int parity, int d, const typename GaugeView<P, recon>::Raw *raw, typename P::real mask)
   {
     using real = typename P::real;
-    constexpr int sign = fwd ? (dagger ? +1 : -1) : (dagger ? -1 : +1);
-    real r[12];
+    constexpr int sign = hop_sign<dagger, fwd>();
+    real r[12], scale;
+    hop_from<P, recon, dagger, fwd, lc, pretwist>(r, scale, arg, in, x, x_cb, parity, d, raw);
     if constexpr (DeferredScale<P>::value) {
-      real scale;
-      hop_from_deferred<P, recon, dagger, fwd, lc, pretwist>(r, scale, arg, in, x, x_cb, parity, d, raw);
       if constexpr (masked) scale *= mask;
       reconstruct_add_scaled(acc, r, d, sign, scale);
     } else {
-      hop_from<P, recon, dagger, fwd, lc, pretwist>(r, arg, in, x, x_cb, parity, d, raw);
       if constexpr (masked) {
 #pragma unroll
         for (int i = 0; i < 12; i++) r[i] *= mask;
@@ -332,17 +353,11 @@ namespace b200
     const Geom &g = arg.geom;
     constexpr bool preload = (kt == K_INTERIOR) && PreloadLinks<P, recon>::value;
     typename GaugeView<P, recon>::Raw raw[preload ? 8 : 1];
-    if constexpr (preload) {
-#pragma unroll
-      for (int d = 0; d < 4; d++) {
-        arg.U.load_raw(raw[2 * d], d, x_cb, parity);
-        arg.U.load_raw(raw[2 * d + 1], d, neighbor_cb<false>(x, g, d), 1 - parity);
-      }
-    }
+    if constexpr (preload) load_links<P, recon>(raw, arg, x, x_cb, parity);
 #pragma unroll
     for (int d = 0; d < 4; d++) {
       { // forward hop: U_d(x) P(d, dagger ? + : -) in(x + d)
-        constexpr int sign = dagger ? +1 : -1;
+        constexpr int sign = hop_sign<dagger, true>();
         const bool ghost = (x[d] + 1 >= g.X[d]) && arg.comm_dim[d];
         real r[12];
         if constexpr (kt == K_INTERIOR) {
@@ -369,7 +384,7 @@ namespace b200
         }
       }
       { // backward hop: U_d(x - d)^dagger P(d, dagger ? - : +) in(x - d)
-        constexpr int sign = dagger ? -1 : +1;
+        constexpr int sign = hop_sign<dagger, false>();
         const bool ghost = (x[d] - 1 < 0) && arg.comm_dim[d];
         real r[12];
         if constexpr (kt == K_INTERIOR) {
@@ -409,32 +424,34 @@ namespace b200
     return inner;
   }
 
-  // Full site update for the interior kernel.
+  // A^{-1} or the twist on the hop sum `acc`, the x term, and the store of one site.  `xf` and `out` are the views of both
+  // parities, so that the multi-RHS kernels can aim the same code at any source; they are indexed by `parity` only where
+  // they are used (indexing them before the hops changes the kernels' instruction schedule).
   //   OP_WILSON    : out = D in                     | xpay: out = x + a D in
   //   OP_CLOVER    : (xpay only)                      out = A x + a D in
   //   OP_CLOVER_PC : out = A^{-1} D in              | xpay: out = x + a A^{-1} D in
-  // With partitioned dims, boundary sites only store their partial sum (the exterior kernel finishes them).
-  template <class P, int recon, bool dagger, bool xpay, OpType op, bool part = true>
-  B2_HD void dslash_site_interior(const DslashArgs<P, recon> &arg, const int *x, int x_cb, int parity)
+  //   OP_TM        : (xpay only)                      out = (1 + i b gamma5) x + a D in
+  //   OP_TM_PC     : out = a (1 + i b gamma5) D in  | xpay: out = x + a (1 + i b gamma5) D in
+  //   OP_TM_PC_PRE : the hops carry the rotation    | xpay: out = x + D in
+  // A site that is not `complete` (a boundary site of the masked interior kernel) has only its local hops: clover-PC and
+  // TM-PC store the bare partial sum, and the exterior kernel applies A^{-1} / the twist and x to the whole sum
+  // (dslash_wilson_clover_preconditioned.cuh:74-101).
+  template <class P, int recon, bool xpay, OpType op>
+  B2_HD void site_epilogue(typename P::real *acc, const DslashArgs<P, recon> &arg, const SpinorView<P> (&xf)[kMaxParity],
+                           const SpinorView<P> (&out)[kMaxParity], int x_cb, int parity, bool complete)
   {
     using real = typename P::real;
-    real acc[24];
-#pragma unroll
-    for (int i = 0; i < 24; i++) acc[i] = 0;
-    wilson_hops<P, recon, dagger, K_INTERIOR, part, op == OP_TM_PC_PRE>(acc, arg, x, x_cb, parity);
-
-    const bool complete = part ? site_is_interior(arg, x) : true;
     if constexpr (op == OP_CLOVER_PC) {
       if (complete) clover_apply_site<P, true>(acc, arg.A, x_cb, parity);
     }
     if constexpr (op == OP_TM_PC) {
-      if (complete) twist_apply(acc, arg.a, arg.twist_b()); // a (1 + i b gamma5) D in
+      if (complete) twist_apply(acc, arg.a, arg.twist_b());
     }
     if constexpr (xpay) {
       real xv[24];
-      arg.x[parity].template load<Cache::STREAM>(xv, x_cb);
+      xf[parity].template load<Cache::STREAM>(xv, x_cb);
       if constexpr (op == OP_CLOVER) clover_apply_site<P, false>(xv, arg.A, x_cb, parity);
-      if constexpr (op == OP_TM) twist_apply(xv, (real)1, arg.twist_b()); // (1 + i b gamma5) x + a D in
+      if constexpr (op == OP_TM) twist_apply(xv, (real)1, arg.twist_b());
       if constexpr (op == OP_TM_PC || op == OP_TM_PC_PRE) { // `a` is the rotation's scale here: plain x + ...
         if (complete) {
 #pragma unroll
@@ -444,10 +461,21 @@ namespace b200
 #pragma unroll
         for (int i = 0; i < 24; i++) acc[i] = xv[i] + arg.a * acc[i];
       }
-      // OP_CLOVER_PC on an incomplete site: store the bare partial sum; x and a are applied by the exterior kernel
-      // after A^{-1} (dslash_wilson_clover_preconditioned.cuh:74-101)
     }
-    arg.out[parity].save(acc, x_cb);
+    out[parity].save(acc, x_cb);
+  }
+
+  // Site update of the interior kernel.  With partitioned dims (`part`), boundary sites only store their partial sum
+  // (the exterior kernel finishes them).
+  template <class P, int recon, bool dagger, bool xpay, OpType op, bool part = true>
+  B2_HD void dslash_site_interior(const DslashArgs<P, recon> &arg, const int *x, int x_cb, int parity)
+  {
+    using real = typename P::real;
+    real acc[24];
+#pragma unroll
+    for (int i = 0; i < 24; i++) acc[i] = 0;
+    wilson_hops<P, recon, dagger, K_INTERIOR, part, op == OP_TM_PC_PRE>(acc, arg, x, x_cb, parity);
+    site_epilogue<P, recon, xpay, op>(acc, arg, arg.x, arg.out, x_cb, parity, part ? site_is_interior(arg, x) : true);
   }
 
   // Complete update of a boundary site once the halo is there: all hops (local or ghost), then clover / xpay exactly as
@@ -461,17 +489,7 @@ namespace b200
 #pragma unroll
     for (int i = 0; i < 24; i++) acc[i] = 0;
     wilson_hops<P, recon, dagger, K_FULL>(acc, arg, x, x_cb, parity);
-    if constexpr (op == OP_CLOVER_PC) clover_apply_site<P, true>(acc, arg.A, x_cb, parity);
-    if constexpr (op == OP_TM_PC) twist_apply(acc, arg.a, arg.twist_b());
-    if constexpr (xpay) {
-      real xv[24];
-      arg.x[parity].template load<Cache::STREAM>(xv, x_cb);
-      if constexpr (op == OP_CLOVER) clover_apply_site<P, false>(xv, arg.A, x_cb, parity);
-      if constexpr (op == OP_TM) twist_apply(xv, (real)1, arg.twist_b());
-#pragma unroll
-      for (int i = 0; i < 24; i++) acc[i] = xv[i] + (op == OP_TM_PC ? acc[i] : arg.a * acc[i]);
-    }
-    arg.out[parity].save(acc, x_cb);
+    site_epilogue<P, recon, xpay, op>(acc, arg, arg.x, arg.out, x_cb, parity, true);
   }
 
   // ------------------------------------------------------------------ multi-RHS (batched) stencil
@@ -485,64 +503,24 @@ namespace b200
     SpinorView<P> out[NS][kMaxParity], in[NS][kMaxParity], x[NS][kMaxParity]; // [source][parity the view holds]
   };
 
+  // the hop of every source: the link part once, the spinor part per source (bit-identical to NS single-source hops)
   template <class P, int recon, bool dagger, bool fwd, int NS>
   B2_HD void hop_local_mrhs(typename P::real (*acc)[24], const DslashArgs<P, recon> &arg, const MrhsFields<P, NS> &f,
                             const int *x, int x_cb, int parity, int d, const typename GaugeView<P, recon>::Raw *raw)
   {
     using real = typename P::real;
-    const Geom &g = arg.geom;
-    constexpr int sign = fwd ? (dagger ? +1 : -1) : (dagger ? -1 : +1);
-    real u[18];
-    real us = (real)1; // deferred link scale (fixed point only)
-    const int n_cb = neighbor_cb<fwd>(x, g, d);
-    if constexpr (DeferredScale<P>::value) {
-      if (raw) {
-        arg.U.unpack_deferred(u, us, *raw, d, fwd ? x_cb : n_cb);
-      } else {
-        typename GaugeView<P, recon>::Raw w;
-        arg.U.load_raw(w, d, fwd ? x_cb : n_cb, fwd ? parity : 1 - parity);
-        arg.U.unpack_deferred(u, us, w, d, fwd ? x_cb : n_cb);
-      }
-    } else {
-      if (raw)
-        arg.U.unpack(u, *raw, d, fwd ? x_cb : n_cb);
-      else if (fwd)
-        arg.U.load(u, d, x_cb, parity);
-      else
-        arg.U.load(u, d, n_cb, 1 - parity);
-    }
+    constexpr int sign = hop_sign<dagger, fwd>();
+    real u[18], us = 1;
+    const int n_cb = neighbor_cb<fwd>(x, arg.geom, d);
+    hop_link<P, recon, fwd, Cache::STREAM>(u, us, arg, x_cb, n_cb, parity, d, raw);
 #pragma unroll
     for (int s = 0; s < NS; s++) {
-      const SpinorView<P> &in = f.in[s][1 - parity];
-      real h[12], r[12];
-      if constexpr (DeferredScale<P>::value) { // same arithmetic as hop_from_deferred (bit-identical per source)
-        const real n = in.load_norm(n_cb);
-        real scale;
-        if (d == 3) {
-          load_spin_pair<P, (sign > 0), Cache::REUSE, false>(h, in, n_cb);
-          scale = (us * n) * (real)2;
-        } else {
-          real v[24];
-          in.template load_planes<0, 24 / P::Ns>(v, n_cb);
-          project(h, v, d, sign);
-          scale = us * n;
-        }
-        su3_mul<!fwd>(r, u, h);
+      real r[12], scale;
+      hop_spinor<P, recon, dagger, fwd>(r, scale, u, us, arg, f.in[s][1 - parity], n_cb, d);
+      if constexpr (DeferredScale<P>::value)
         reconstruct_add_scaled(acc[s], r, d, sign, scale);
-      } else {
-        if (d == 3) {
-          real t[12];
-          load_spin_pair<P, (sign > 0)>(t, in, n_cb);
-#pragma unroll
-          for (int i = 0; i < 12; i++) h[i] = 2 * t[i];
-        } else {
-          real v[24];
-          in.load(v, n_cb);
-          project(h, v, d, sign);
-        }
-        su3_mul<!fwd>(r, u, h);
+      else
         reconstruct_add(acc[s], r, d, sign);
-      }
     }
   }
 
@@ -552,7 +530,6 @@ namespace b200
   B2_HD void dslash_site_mrhs(const DslashArgs<P, recon> &arg, const MrhsFields<P, NS> &f, const int *x, int x_cb, int parity)
   {
     using real = typename P::real;
-    const Geom &g = arg.geom;
     real acc[NS][24];
 #pragma unroll
     for (int s = 0; s < NS; s++)
@@ -561,30 +538,14 @@ namespace b200
 
     constexpr bool preload = PreloadLinks<P, recon>::value;
     typename GaugeView<P, recon>::Raw raw[preload ? 8 : 1];
-    if constexpr (preload) {
-#pragma unroll
-      for (int d = 0; d < 4; d++) {
-        arg.U.load_raw(raw[2 * d], d, x_cb, parity);
-        arg.U.load_raw(raw[2 * d + 1], d, neighbor_cb<false>(x, g, d), 1 - parity);
-      }
-    }
+    if constexpr (preload) load_links<P, recon>(raw, arg, x, x_cb, parity);
 #pragma unroll
     for (int d = 0; d < 4; d++) {
       hop_local_mrhs<P, recon, dagger, true, NS>(acc, arg, f, x, x_cb, parity, d, preload ? &raw[2 * d] : nullptr);
       hop_local_mrhs<P, recon, dagger, false, NS>(acc, arg, f, x, x_cb, parity, d, preload ? &raw[2 * d + 1] : nullptr);
     }
 #pragma unroll
-    for (int s = 0; s < NS; s++) {
-      if constexpr (op == OP_CLOVER_PC) clover_apply_site<P, true>(acc[s], arg.A, x_cb, parity);
-      if constexpr (xpay) {
-        real xv[24];
-        f.x[s][parity].template load<Cache::STREAM>(xv, x_cb);
-        if constexpr (op == OP_CLOVER) clover_apply_site<P, false>(xv, arg.A, x_cb, parity);
-#pragma unroll
-        for (int i = 0; i < 24; i++) acc[s][i] = xv[i] + arg.a * acc[s][i];
-      }
-      f.out[s][parity].save(acc[s], x_cb);
-    }
+    for (int s = 0; s < NS; s++) site_epilogue<P, recon, xpay, op>(acc[s], arg, f.x[s], f.out[s], x_cb, parity, true);
   }
 
   // Multi-RHS, CTA flavour: one thread = one (site, source) pair, the sources of a site sit in the same CTA
@@ -602,24 +563,19 @@ namespace b200
                              const SpinorView<P> &xf, const int *x, int x_cb, int parity)
   {
     using real = typename P::real;
-    const Geom &g = arg.geom;
     real acc[24];
 #pragma unroll
     for (int i = 0; i < 24; i++) acc[i] = 0;
     constexpr bool preload = preload_links && PreloadLinks<P, recon>::value;
     typename GaugeView<P, recon>::Raw raw[preload ? 8 : 1];
-    if constexpr (preload) {
-#pragma unroll
-      for (int d = 0; d < 4; d++) {
-        arg.U.template load_raw<lc>(raw[2 * d], d, x_cb, parity);
-        arg.U.template load_raw<lc>(raw[2 * d + 1], d, neighbor_cb<false>(x, g, d), 1 - parity);
-      }
-    }
+    if constexpr (preload) load_links<P, recon, lc>(raw, arg, x, x_cb, parity);
 #pragma unroll
     for (int d = 0; d < 4; d++) {
       hop_add<P, recon, dagger, true, false, lc>(acc, arg, in, x, x_cb, parity, d, preload ? &raw[2 * d] : nullptr, (real)1);
       hop_add<P, recon, dagger, false, false, lc>(acc, arg, in, x, x_cb, parity, d, preload ? &raw[2 * d + 1] : nullptr, (real)1);
     }
+    // site_epilogue for the multi-RHS ops, on the views the kernel indexed at entry: handing site_epilogue both parities
+    // would index them after the hops instead, and change the CTA kernels' instruction schedule
     if constexpr (op == OP_CLOVER_PC) clover_apply_site<P, true>(acc, arg.A, x_cb, parity);
     if constexpr (xpay) {
       real xv[24];
@@ -645,21 +601,12 @@ namespace b200
     if constexpr (op == OP_CLOVER_PC || op == OP_TM_PC) {
 #pragma unroll
       for (int i = 0; i < 24; i++) acc[i] += partial[i];
-      if constexpr (op == OP_CLOVER_PC)
-        clover_apply_site<P, true>(acc, arg.A, x_cb, parity);
-      else
-        twist_apply(acc, arg.a, arg.twist_b());
-      if constexpr (xpay) {
-        real xv[24];
-        arg.x[parity].template load<Cache::STREAM>(xv, x_cb);
-#pragma unroll
-        for (int i = 0; i < 24; i++) acc[i] = xv[i] + (op == OP_TM_PC ? acc[i] : arg.a * acc[i]);
-      }
+      site_epilogue<P, recon, xpay, op>(acc, arg, arg.x, arg.out, x_cb, parity, true);
     } else {
 #pragma unroll
       for (int i = 0; i < 24; i++) acc[i] = partial[i] + (xpay ? arg.a * acc[i] : acc[i]);
+      arg.out[parity].save(acc, x_cb);
     }
-    arg.out[parity].save(acc, x_cb);
   }
 
   // Fused-exterior thread -> (dim, face, face index) decode and the corner-ownership rule: a boundary site that lies

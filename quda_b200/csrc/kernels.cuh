@@ -530,21 +530,22 @@ namespace b200
     for (int i = 0; i < pl.n; i++) {
       const LaunchStep &l = pl.step[i];
       const dim3 grid(l.grid[0], l.grid[1], l.grid[2]);
-      switch (l.kind) {
-      case LAUNCH_INTERIOR:
-        if (l.masked)
-          dslash_interior_kernel<P, recon, dagger, xpay, op, true><<<grid, l.threads, 0, s>>>(arg, l.tm);
-        else
-          dslash_interior_kernel<P, recon, dagger, xpay, op, false><<<grid, l.threads, 0, s>>>(arg, l.tm);
-        break;
-      case LAUNCH_BOUNDARY: dslash_boundary_kernel<P, recon, dagger, xpay, op><<<grid, l.threads, 0, s>>>(arg, l.tm, l.st); break;
-      case LAUNCH_EXTERIOR: dslash_exterior_kernel<P, recon, dagger, xpay, op><<<grid, l.threads, 0, s>>>(arg); break;
-      case LAUNCH_FUSED: {
-        PackArgs<P> pk {};
-        if (rq.fused_pack) fill_pack_args(pk, *rq.fused_pack);
-        dslash_fused_kernel<P, recon, dagger, xpay, op><<<grid, l.threads, 0, s>>>(arg, l.tm, pk, l.fs);
-        break;
-      }
+      if (l.kind == LAUNCH_INTERIOR && !l.masked) {
+        dslash_interior_kernel<P, recon, dagger, xpay, op, false><<<grid, l.threads, 0, s>>>(arg, l.tm);
+      } else if constexpr (!has_partitioned_kernels(op)) {
+        return refuse_partitioned_tm_pc_pre();
+      } else {
+        switch (l.kind) {
+        case LAUNCH_INTERIOR: dslash_interior_kernel<P, recon, dagger, xpay, op, true><<<grid, l.threads, 0, s>>>(arg, l.tm); break;
+        case LAUNCH_BOUNDARY: dslash_boundary_kernel<P, recon, dagger, xpay, op><<<grid, l.threads, 0, s>>>(arg, l.tm, l.st); break;
+        case LAUNCH_EXTERIOR: dslash_exterior_kernel<P, recon, dagger, xpay, op><<<grid, l.threads, 0, s>>>(arg); break;
+        case LAUNCH_FUSED: {
+          PackArgs<P> pk {};
+          if (rq.fused_pack) fill_pack_args(pk, *rq.fused_pack);
+          dslash_fused_kernel<P, recon, dagger, xpay, op><<<grid, l.threads, 0, s>>>(arg, l.tm, pk, l.fs);
+          break;
+        }
+        }
       }
       count_launch();
     }

@@ -326,6 +326,15 @@ namespace b200
     }
   }
 
+  // The symmetric preconditioned twisted-mass dagger rotates the neighbour spinors before the hop.  The pack kernel does
+  // not rotate the faces it sends, so this op is refused on a partitioned lattice and has no partitioned kernels
+  // (plan.h::has_partitioned_kernels).
+  inline int refuse_partitioned_tm_pc_pre()
+  {
+    return set_error(B200_ERR_UNSUPPORTED, "symmetric preconditioned twisted-mass dagger on a partitioned lattice needs the "
+                                           "twist in the pack kernel: not built");
+  }
+
   // Validate a b200_dslash_args block and turn it into the precision-erased launch request
   // (shared by the CUDA library and the test-only host twin so both see identical argument semantics).
   inline int make_request(LaunchRequest &rq, const b200_dslash_args *a, bool &nothing_to_do)
@@ -353,9 +362,7 @@ namespace b200
       if (a->asymmetric && !a->dagger) return set_error(B200_ERR_INVALID, "asymmetric operator only defined for dagger");
       if (a->asymmetric && a->x.v) return set_error(B200_ERR_INVALID, "asymmetric operator not defined for xpay");
       if (a->out.n_parity != 1) return set_error(B200_ERR_INVALID, "Preconditioned twisted-mass operator not defined nParity=2");
-      if (a->dagger && !a->asymmetric && any_comm_tm)
-        return set_error(B200_ERR_UNSUPPORTED, "symmetric preconditioned twisted-mass dagger on a partitioned lattice needs the "
-                                               "twist in the pack kernel: not built");
+      if (a->dagger && !a->asymmetric && any_comm_tm) return refuse_partitioned_tm_pc_pre();
     }
     if (a->op == B200_OP_CLOVER_PC && a->out.n_parity != 1)
       return set_error(B200_ERR_INVALID, "preconditioned clover operator only defined on single-parity fields");

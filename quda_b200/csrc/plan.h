@@ -207,6 +207,10 @@ namespace b200
     bool whole;         // the steps update every site of the operator
   };
 
+  // OP_TM_PC_PRE (symmetric preconditioned twisted-mass dagger) is refused on a partitioned lattice (make_request), so
+  // the executors build no masked-interior, boundary, exterior or fused step for it.
+  constexpr bool has_partitioned_kernels(OpType op) { return op != OP_TM_PC_PRE; }
+
   // The launches of one Dslash request for the kernel arguments `arg` (DslashArgs of any precision / reconstruct)
   template <class Arg> int plan_dslash(LaunchPlan &pl, const LaunchRequest &rq, const Arg &arg)
   {

@@ -523,13 +523,13 @@ namespace b200
     for (int i = 0; i < GV::M; i++) raw.w[i] = lds<typename GV::V>(rec + i * row_bytes);
   }
 
-  // One hop with the neighbour spinor in shared memory and the link already unpacked; arithmetic identical to hop_from
+  // One hop with the neighbour spinor in shared memory and the link already unpacked; arithmetic identical to hop_spinor
   // (dslash_site.h) operation for operation.
   template <class P, bool dagger, bool fwd, int d>
   B2_HD void tma_hop(typename P::real *acc, const typename P::real *u, sptr spinor_rec, int srow_bytes)
   {
     using real = typename P::real;
-    constexpr int sign = fwd ? (dagger ? +1 : -1) : (dagger ? -1 : +1);
+    constexpr int sign = hop_sign<dagger, fwd>();
     real h[12], r[12];
     if constexpr (d == 3) {
       constexpr int np = 12 / P::Ns;
@@ -632,27 +632,11 @@ namespace b200
     }
   }
 
-  // clover / twist / xpay epilogue and store: the `complete` branch of dslash_site_interior (unpartitioned lattice)
+  // clover / xpay epilogue and store of a TMA site: every site of the (unpartitioned) lattice is complete
   template <class P, int recon, bool dagger, bool xpay, OpType op>
   B2_HD void tma_epilogue(typename P::real *acc, const DslashArgs<P, recon> &arg, int x_cb, int parity)
   {
-    using real = typename P::real;
-    if constexpr (op == OP_CLOVER_PC) clover_apply_site<P, true>(acc, arg.A, x_cb, parity);
-    if constexpr (op == OP_TM_PC) twist_apply(acc, arg.a, arg.twist_b());
-    if constexpr (xpay) {
-      real xv[24];
-      arg.x[parity].template load<Cache::STREAM>(xv, x_cb);
-      if constexpr (op == OP_CLOVER) clover_apply_site<P, false>(xv, arg.A, x_cb, parity);
-      if constexpr (op == OP_TM) twist_apply(xv, (real)1, arg.twist_b());
-      if constexpr (op == OP_TM_PC) {
-#pragma unroll
-        for (int i = 0; i < 24; i++) acc[i] = xv[i] + acc[i];
-      } else {
-#pragma unroll
-        for (int i = 0; i < 24; i++) acc[i] = xv[i] + arg.a * acc[i];
-      }
-    }
-    arg.out[parity].save(acc, x_cb);
+    site_epilogue<P, recon, xpay, op>(acc, arg, arg.x, arg.out, x_cb, parity, true);
   }
 
 } // namespace b200

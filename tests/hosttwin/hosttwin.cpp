@@ -8,6 +8,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <numeric>
+#include <type_traits>
 #include <vector>
 
 #include "../../quda_b200/csrc/plan.h"
@@ -97,27 +98,31 @@ namespace b200
       prev = hits[(size_t)par * g.volume_cb + x_cb]++;
       return prev != 0;
     };
+    // dslash_interior_kernel<..., part> over the box of step l
+    auto interior = [&](const LaunchStep &l, auto part) {
+      long rep = 0;
+#pragma omp parallel for collapse(2) reduction(+ : rep)
+      for (int bz = 0; bz < l.grid[2]; bz++)
+        for (int by = 0; by < l.grid[1]; by++)
+          for (int bx = 0; bx < l.grid[0]; bx++)
+            for (int tid = 0; tid < l.threads; tid++) {
+              int x[4], x_cb, par;
+              if (!tile_site(x, x_cb, par, g, l.tm, arg.n_parity, arg.parity, bx, by, bz, tid)) continue;
+              dslash_site_interior<P, recon, dagger, xpay, op, decltype(part)::value>(arg, x, x_cb, par);
+              rep += twice(par, x_cb);
+            }
+      return rep;
+    };
     long repeats = 0;
     for (int i = 0; i < pl.n; i++) {
       const LaunchStep &l = pl.step[i];
-      const TileMap &tm = l.tm;
-      if (l.kind == LAUNCH_INTERIOR) {
-#pragma omp parallel for collapse(2) reduction(+ : repeats)
-        for (int bz = 0; bz < l.grid[2]; bz++)
-          for (int by = 0; by < l.grid[1]; by++)
-            for (int bx = 0; bx < l.grid[0]; bx++)
-              for (int tid = 0; tid < l.threads; tid++) {
-                int x[4], x_cb, par;
-                if (!tile_site(x, x_cb, par, g, tm, arg.n_parity, arg.parity, bx, by, bz, tid)) continue;
-                if (l.masked)
-                  dslash_site_interior<P, recon, dagger, xpay, op, true>(arg, x, x_cb, par);
-                else
-                  dslash_site_interior<P, recon, dagger, xpay, op, false>(arg, x, x_cb, par);
-                repeats += twice(par, x_cb);
-              }
-        continue;
-      }
-      if (l.kind == LAUNCH_FUSED) {
+      if (l.kind == LAUNCH_INTERIOR && !l.masked) {
+        repeats += interior(l, std::false_type {});
+      } else if constexpr (!has_partitioned_kernels(op)) {
+        return refuse_partitioned_tm_pc_pre();
+      } else if (l.kind == LAUNCH_INTERIOR) {
+        repeats += interior(l, std::true_type {});
+      } else if (l.kind == LAUNCH_FUSED) {
         // dslash_fused_kernel: the pack CTAs first (all faces land before any boundary CTA waits), then blocks n_pack + b
         const FusedShape &fs = l.fs;
         if (fs.n_pack) {
@@ -143,7 +148,7 @@ namespace b200
           for (int tid = 0; tid < l.threads; tid++) {
             int x[4], x_cb, par = arg.parity;
             if (ib >= 0) {
-              if (!tile_site(x, x_cb, par, g, tm, arg.n_parity, arg.parity, bx, by, bz, tid) || !site_is_interior(arg, x)) continue;
+              if (!tile_site(x, x_cb, par, g, l.tm, arg.n_parity, arg.parity, bx, by, bz, tid) || !site_is_interior(arg, x)) continue;
               dslash_site_interior<P, recon, dagger, xpay, op, false>(arg, x, x_cb, par);
             } else {
               const int t = (b - fs.n_interior_first) * l.threads + tid;
@@ -153,25 +158,25 @@ namespace b200
             repeats += twice(par, x_cb);
           }
         }
-        continue;
-      }
-      if (int rc = check_halo_arrived(arg)) return rc;
-      for (int by = 0; by < l.grid[1]; by++) {
-        const int par = arg.n_parity == 2 ? by : arg.parity;
+      } else {
+        if (int rc = check_halo_arrived(arg)) return rc;
+        for (int by = 0; by < l.grid[1]; by++) {
+          const int par = arg.n_parity == 2 ? by : arg.parity;
 #pragma omp parallel for reduction(+ : repeats)
-        for (int bx = 0; bx < l.grid[0]; bx++)
-          for (int tid = 0; tid < l.threads; tid++) {
-            int x[4], x_cb;
-            if (l.kind == LAUNCH_BOUNDARY) {
-              if (!slab_site(x, x_cb, g, tm, l.st, par, bx, tid)) continue;
-              dslash_site_full<P, recon, dagger, xpay, op>(arg, x, x_cb, par);
-            } else {
-              const int t = bx * l.threads + tid;
-              if (t >= arg.threads_ext[4] || !exterior_thread_site(x, x_cb, arg, t, par)) continue;
-              dslash_site_exterior<P, recon, dagger, xpay, op>(arg, x, x_cb, par);
+          for (int bx = 0; bx < l.grid[0]; bx++)
+            for (int tid = 0; tid < l.threads; tid++) {
+              int x[4], x_cb;
+              if (l.kind == LAUNCH_BOUNDARY) {
+                if (!slab_site(x, x_cb, g, l.tm, l.st, par, bx, tid)) continue;
+                dslash_site_full<P, recon, dagger, xpay, op>(arg, x, x_cb, par);
+              } else {
+                const int t = bx * l.threads + tid;
+                if (t >= arg.threads_ext[4] || !exterior_thread_site(x, x_cb, arg, t, par)) continue;
+                dslash_site_exterior<P, recon, dagger, xpay, op>(arg, x, x_cb, par);
+              }
+              repeats += twice(par, x_cb);
             }
-            repeats += twice(par, x_cb);
-          }
+        }
       }
     }
     if (repeats) return set_error(B200_ERR_INVALID, "the launch plan updates %ld sites more than once", repeats);
