@@ -329,6 +329,28 @@ int b200_invert_cg(b200_dirac *precise, b200_dirac *sloppy, const b200_spinor *x
  * same fields and precisions as b200_invert_cg, restarts after a breakdown are counted in reliable_updates */
 int b200_invert_bicgstab(b200_dirac *precise, b200_dirac *sloppy, const b200_spinor *x, const b200_spinor *b, b200_solver_param *param);
 
+#define B200_MAX_SHIFTS 32 /* shifts of one multi-shift solve (QUDA_MAX_MULTI_SHIFT) */
+typedef struct {
+  int n_shift;                              /* 1 .. B200_MAX_SHIFTS */
+  double offset[B200_MAX_SHIFTS];           /* sigma_j: finite, non-decreasing */
+  double tol_offset[B200_MAX_SHIFTS];       /* per-shift relative residual target, > 0 */
+  int maxiter;                              /* of the multi-shift loop and of each refinement solve */
+  double delta;                             /* reliable-update threshold */
+  int iter;                                 /* out: multi-shift iterations */
+  int iter_offset[B200_MAX_SHIFTS];         /* out: iteration at which shift j retired */
+  int refine_iter[B200_MAX_SHIFTS];         /* out: iterations of shift j's single-shift refinement (0: none needed) */
+  double iter_res_offset[B200_MAX_SHIFTS];  /* out: iterated residual zeta_j |r| / |b| when shift j retired */
+  double true_res_offset[B200_MAX_SHIFTS];  /* out: |b - (A + sigma_j) x_j| / |b| in the precise operator */
+  int reliable_updates;
+  double secs, gflops;
+  int host_syncs;
+} b200_multishift_param;
+/* Multi-shift CG: (MdagM + sigma_j) x_j = b for every shift at once (the preconditioned system for the *pc types, the full one
+ * otherwise).  x points to n_shift descriptors; every x_j is overwritten (the initial guess is ignored).  Shifts whose true
+ * residual misses tol_offset[j] are refined by a single-shift solve from x_j. */
+int b200_invert_multishift_cg(b200_dirac *precise, b200_dirac *sloppy, const b200_spinor *x, const b200_spinor *b,
+                              b200_multishift_param *param);
+
 const char *b200_last_error(void);
 int b200_abi_version(void);
 /* number of kernels this library has launched since load (bench.py's gpu_launches evidence) */

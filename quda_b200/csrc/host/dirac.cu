@@ -1,9 +1,12 @@
 // Implementation of the host-side operator / blas / solver layer (design notes and reference citations: dirac.h).
+#include <algorithm>
 #include <chrono>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
+#include <cstdint>
 #include <cstring>
+#include <deque>
 #include <map>
 #include <memory>
 #include <type_traits>
@@ -799,10 +802,209 @@ namespace b200
       template <int N> struct Scalars {
         double s[N];
       };
-      // the whole scalar block of a solver (N <= 32)
+      // the whole scalar block of a solver (one thread per scalar)
       template <int N> __global__ void set_scalars_kernel(double *S, Scalars<N> v)
       {
         if (threadIdx.x < N) S[threadIdx.x] = v.s[threadIdx.x];
+      }
+
+      // ---- multi-shift CG: one scalar block for all shifts.  Per-shift arrays of B200_MAX_SHIFTS entries; shift 0 is the
+      // unshifted recursion (zeta_0 = 1, alpha_0 / beta_0 are CG's alpha / beta).  The active shifts are always the prefix
+      // j < M_NACT: a shift retires only after every shift above it has.
+      constexpr int kShifts = B200_MAX_SHIFTS;
+      enum MsScalar {
+        M_R2 = 0, M_R2_OLD = 1, M_PAP = 2,
+        M_NACT = 3,    // active shifts
+        M_NUPD = 4,    // shifts the x / p update of this iteration touches (M_NACT before this iteration's retirements)
+        M_DONE = 5,    // 1 once every shift has retired: every multi-shift kernel after that returns at once
+        M_ITER = 6,    // iterations completed (|r|^2 finalisers run)
+        M_RAW = 7,     // the global sum of the last reduction
+        M_DSIG = 16,                   // sigma_j - sigma_0
+        M_ZETA = M_DSIG + kShifts,     // zeta_j
+        M_ZOLD = M_ZETA + kShifts,     // zeta_j of the previous iteration
+        M_ALPHA = M_ZOLD + kShifts,    // alpha_j
+        M_BETA = M_ALPHA + kShifts,    // beta_j
+        M_STOP = M_BETA + kShifts,     // stopping value of |r_j|^2
+        M_RES = M_STOP + kShifts,      // |r_j|^2 = zeta_j^2 |r|^2, frozen when shift j retires
+        M_RETIRED = M_RES + kShifts,   // iteration at which shift j retired (-1: still active)
+        M_COUNT = M_RETIRED + kShifts
+      };
+      // Derive the multi-shift scalars from the global sum in S[M_RAW] (the CG-M recursion, lib/inv_multi_cg_quda.cpp):
+      //   FIN_PAP  v = <p_0, (A + sigma_0) p_0>   alpha_0 = r2 / v; for the active shifts zeta_j, zeta_old_j, alpha_j
+      //                                          (updateAlphaZeta, :170-186); M_NUPD <- M_NACT
+      //   FIN_R2   v = |r|^2                     r2_old <- r2, r2 <- v, beta_0 = v / r2_old,
+      //                                          beta_j = beta_0 zeta_j alpha_j / (zeta_old_j alpha_0) (:100, :380); then retire
+      //                                          shifts from the top while zeta_j^2 r2 <= stop_j (:394-409), done when none is left
+      // Zero divisors give zero, never NaN; a shift with zeta_j = 0 has converged.  Products are rounded one by one
+      // (mul_rn), so the device and the host derive bit-identical scalars.
+      __host__ __device__ inline void ms_scalars(double *S, int fin)
+      {
+        double *dsig = S + M_DSIG, *zeta = S + M_ZETA, *zold = S + M_ZOLD, *alpha = S + M_ALPHA, *beta = S + M_BETA;
+        const double v = S[M_RAW];
+        int n = (int)S[M_NACT];
+        if (fin == FIN_PAP) {
+          const double a_old = alpha[0], b_old = beta[0];
+          const double a0 = v != 0.0 ? S[M_R2] / v : 0.0;
+          S[M_PAP] = v;
+          alpha[0] = a0;
+          for (int j = 1; j < n; j++) {
+            const double c0 = mul_rn(mul_rn(zeta[j], zold[j]), a_old);
+            const double c1 = mul_rn(mul_rn(a0, b_old), zold[j] - zeta[j]);
+            const double c2 = mul_rn(mul_rn(zold[j], a_old), 1.0 + mul_rn(dsig[j], a0));
+            const double den = c1 + c2;
+            zold[j] = zeta[j];
+            zeta[j] = den != 0.0 ? c0 / den : 0.0;
+            alpha[j] = zeta[j] != 0.0 ? mul_rn(a0, zeta[j]) / zold[j] : 0.0; // zeta_j != 0 needs c0 != 0, so zold_j != 0
+          }
+          S[M_NUPD] = n;
+        } else if (fin == FIN_R2) {
+          const double old = S[M_R2];
+          S[M_R2_OLD] = old;
+          S[M_R2] = v;
+          const double b0 = old != 0.0 ? v / old : 0.0;
+          beta[0] = b0;
+          for (int j = 1; j < n; j++) {
+            const double den = mul_rn(zold[j], alpha[0]);
+            beta[j] = den != 0.0 ? mul_rn(mul_rn(b0, zeta[j]), alpha[j]) / den : 0.0;
+          }
+          S[M_ITER] += 1.0;
+          for (int j = 0; j < n; j++) S[M_RES + j] = mul_rn(mul_rn(zeta[j], zeta[j]), v);
+          while (n > 0 && S[M_RES + n - 1] <= S[M_STOP + n - 1]) {
+            n--;
+            S[M_RETIRED + n] = S[M_ITER];
+          }
+          S[M_NACT] = n;
+          if (n == 0) S[M_DONE] = 1.0;
+        }
+      }
+      struct MsTraits {
+        static constexpr int kVals = 1, kCount = M_COUNT, kRaw = M_RAW;
+        __host__ __device__ static void derive(double *S, int fin) { ms_scalars(S, fin); }
+      };
+
+      // The multi-shift kernels move 16 bytes per access: 2 doubles or 4 floats.  Both native orders keep the field a
+      // flat array of reals and the kernels act element-wise, so element i of every field is the same component.
+      template <typename T> struct alignas(16) Vec {
+        static constexpr int W = 16 / sizeof(T);
+        T e[W];
+      };
+      // the x and p fields of every shift, by value
+      template <typename T> struct MsFields {
+        T *x[kShifts];
+        T *p[kShifts];
+      };
+      __device__ __forceinline__ void ms_finish(double acc, const ReduceArgs &ra)
+      {
+        __shared__ double wb[kThreads / 32];
+        const double s = block_sum(acc, wb);
+        finish_reduction<1, MsTraits>(&s, ra.partials, ra.ticket, ra.S, ra.host_out, ra.fin, ra.peers);
+      }
+      // Ap += sigma_0 p ; <p, Ap>   (finaliser FIN_PAP).  Once M_DONE is set it returns at once, and clears M_NUPD so
+      // that the x / p update queued behind it does nothing either.
+      template <typename T>
+      __global__ void __launch_bounds__(kThreads) ms_dot_kernel(const Vec<T> *__restrict__ p, Vec<T> *__restrict__ Ap, double sigma,
+                                                                size_t n, ReduceArgs ra)
+      {
+        if (ra.S[M_DONE] != 0.0) {
+          if (blockIdx.x == 0 && threadIdx.x == 0) ra.S[M_NUPD] = 0.0;
+          return;
+        }
+        double acc = 0;
+        for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+          const Vec<T> pv = p[i];
+          Vec<T> av = Ap[i];
+#pragma unroll
+          for (int e = 0; e < Vec<T>::W; e++) {
+            av.e[e] = (T)((double)av.e[e] + sigma * (double)pv.e[e]);
+            acc += (double)pv.e[e] * (double)av.e[e];
+          }
+          if (sigma != 0.0) Ap[i] = av;
+        }
+        ms_finish(acc, ra);
+      }
+      // r -= alpha_0 Ap ; |r|^2   (finaliser FIN_R2: beta_j, retirement, done flag)
+      template <typename T>
+      __global__ void __launch_bounds__(kThreads) ms_update_r_kernel(Vec<T> *__restrict__ r, const Vec<T> *__restrict__ Ap, size_t n,
+                                                                     ReduceArgs ra)
+      {
+        if (ra.S[M_DONE] != 0.0) return;
+        const double alpha = ra.S[M_ALPHA];
+        double acc = 0;
+        for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+          const Vec<T> av = Ap[i];
+          Vec<T> rv = r[i];
+#pragma unroll
+          for (int e = 0; e < Vec<T>::W; e++) {
+            rv.e[e] = (T)((double)rv.e[e] - alpha * (double)av.e[e]);
+            acc += (double)rv.e[e] * (double)rv.e[e];
+          }
+          r[i] = rv;
+        }
+        ms_finish(acc, ra);
+      }
+      // The hot path: for every shift j < M_NUPD, x_j += alpha_j p_j ; p_j = zeta_j r + beta_j p_j (shift 0: zeta = 1, the
+      // reference's axpyZpbx; the others its axpyBzpcx).  r is read once per element; a retired shift costs no bytes:
+      // (1 + 4 M_NUPD) fields of traffic.
+      template <typename T>
+      __global__ void __launch_bounds__(kThreads) ms_update_xp_kernel(MsFields<T> f, const Vec<T> *__restrict__ r, size_t n,
+                                                                      const double *__restrict__ S)
+      {
+        __shared__ double c[3][kShifts]; // alpha_j, zeta_j, beta_j
+        const int ns = (int)S[M_NUPD];
+        if (ns == 0) return;
+        const int t = threadIdx.x;
+        if (t < ns) {
+          c[0][t] = S[M_ALPHA + t];
+          c[1][t] = S[M_ZETA + t];
+          c[2][t] = S[M_BETA + t];
+        }
+        __syncthreads();
+        for (size_t i = (size_t)blockIdx.x * blockDim.x + t; i < n; i += (size_t)gridDim.x * blockDim.x) {
+          const Vec<T> rv = r[i];
+          for (int j = 0; j < ns; j++) {
+            Vec<T> *x = reinterpret_cast<Vec<T> *>(f.x[j]), *p = reinterpret_cast<Vec<T> *>(f.p[j]);
+            const double a = c[0][j], z = c[1][j], b = c[2][j];
+            Vec<T> xv = x[i], pv = p[i];
+#pragma unroll
+            for (int e = 0; e < Vec<T>::W; e++) {
+              const double pe = pv.e[e];
+              xv.e[e] = (T)((double)xv.e[e] + a * pe);
+              pv.e[e] = (T)(z * (double)rv.e[e] + b * pe);
+            }
+            x[i] = xv;
+            p[i] = pv;
+          }
+        }
+      }
+      // After a reliable update: d = r_new - r ; p_0 += d, p_j += zeta_j d for the active shifts ; r = r_new.  That keeps
+      // p_j = zeta_j r_new + beta_j p_j,old exactly (CG's late-update repair, per shift).  It also stores the true |r|^2,
+      // clears M_DONE and reopens shift 0 if every shift had retired; the blocks that read M_NACT before or after
+      // block 0 rewrites it get the same count.
+      template <typename T>
+      __global__ void __launch_bounds__(kThreads) ms_replace_r_kernel(MsFields<T> f, Vec<T> *__restrict__ r, const Vec<T> *__restrict__ r_new,
+                                                                      size_t n, double *S, double r2)
+      {
+        __shared__ double z[kShifts];
+        const int ns = max((int)S[M_NACT], 1);
+        const int t = threadIdx.x;
+        if (t < ns) z[t] = t == 0 ? 1.0 : S[M_ZETA + t];
+        __syncthreads();
+        if (blockIdx.x == 0 && t == 0) {
+          S[M_NACT] = ns;
+          S[M_DONE] = 0.0;
+          S[M_R2] = r2;
+        }
+        for (size_t i = (size_t)blockIdx.x * blockDim.x + t; i < n; i += (size_t)gridDim.x * blockDim.x) {
+          const Vec<T> rn = r_new[i], ro = r[i];
+          for (int j = 0; j < ns; j++) {
+            Vec<T> *p = reinterpret_cast<Vec<T> *>(f.p[j]);
+            Vec<T> pv = p[i];
+#pragma unroll
+            for (int e = 0; e < Vec<T>::W; e++) pv.e[e] = (T)((double)pv.e[e] + z[j] * ((double)rn.e[e] - (double)ro.e[e]));
+            p[i] = pv;
+          }
+          r[i] = rn;
+        }
       }
 
       static void check_pair(const ColorSpinorField &x, const ColorSpinorField &y)
@@ -863,7 +1065,7 @@ namespace b200
       }
       template <typename Tr> static void set_all(const Exec &ex, const Scalars<Tr::kCount> &s)
       {
-        set_scalars_kernel<Tr::kCount><<<1, 32, 0, cs(ex.stream)>>>(workspace<Tr>(ex.stream).scalars, s);
+        set_scalars_kernel<Tr::kCount><<<1, (Tr::kCount + 31) / 32 * 32, 0, cs(ex.stream)>>>(workspace<Tr>(ex.stream).scalars, s);
         cuda_ok(cudaGetLastError(), "scalar launch");
       }
       // Launch one reduction of nv sums with finaliser fin into the scalar block of Tr (kernel(T(), ra) launches it).
@@ -1046,6 +1248,74 @@ namespace b200
           using T = decltype(t);
           bicg_update_p_kernel<T><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(p.data<T>(), r.data<T>(), v.data<T>(), n, S);
         });
+      }
+
+      // ---- multi-shift CG iteration pieces (used by invertMultiShiftCG below); all operands share the sloppy precision
+      template <typename T> static const Vec<T> *vec(const ColorSpinorField &f) { return reinterpret_cast<const Vec<T> *>(f.v); }
+      template <typename T> static Vec<T> *vec(ColorSpinorField &f) { return reinterpret_cast<Vec<T> *>(f.v); }
+      template <typename... F> static size_t ms_check(const ColorSpinorField &x, const F &...ys)
+      {
+        check_same(x, ys...);
+        for (const ColorSpinorField *f : {&x, &ys...})
+          if (reinterpret_cast<uintptr_t>(f->v) % 16) throw Error("multi-shift CG: fields must be 16-byte aligned");
+        return x.Length(); // a multiple of 24 reals, so of every vector width
+      }
+      template <typename T> static MsFields<T> ms_fields(const std::vector<ColorSpinorField> &x, const std::vector<ColorSpinorField> &p)
+      {
+        MsFields<T> f {};
+        for (size_t j = 0; j < p.size(); j++) {
+          if (j < x.size()) f.x[j] = x[j].data<T>();
+          f.p[j] = p[j].data<T>();
+        }
+        return f;
+      }
+      static Pending ms_dot(const ColorSpinorField &p, ColorSpinorField &Ap, double sigma, const Exec &ex, int &syncs)
+      {
+        const size_t n = ms_check(p, Ap);
+        return reduce<MsTraits>(ex, 1, FIN_PAP, syncs, p.precision, 4 * (long long)n, [&](auto t, const ReduceArgs &ra) {
+          using T = decltype(t);
+          ms_dot_kernel<T><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(vec<T>(p), vec<T>(Ap), sigma, n / Vec<T>::W, ra);
+        });
+      }
+      static Pending ms_update_r(ColorSpinorField &r, const ColorSpinorField &Ap, const Exec &ex, int &syncs)
+      {
+        const size_t n = ms_check(r, Ap);
+        return reduce<MsTraits>(ex, 1, FIN_R2, syncs, r.precision, 4 * (long long)n, [&](auto t, const ReduceArgs &ra) {
+          using T = decltype(t);
+          ms_update_r_kernel<T><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(vec<T>(r), vec<T>(Ap), n / Vec<T>::W, ra);
+        });
+      }
+      // n_active: the host's view of the active shifts, for the flop count only (the kernel reads M_NUPD)
+      static void ms_update_xp(const std::vector<ColorSpinorField> &x, const std::vector<ColorSpinorField> &p, const ColorSpinorField &r,
+                               int n_active, const Exec &ex)
+      {
+        size_t n = 0;
+        for (size_t j = 0; j < p.size(); j++) n = ms_check(r, x[j], p[j]);
+        const double *S = workspace<MsTraits>(ex.stream).scalars;
+        launch(r.precision, 5 * (long long)n * n_active, [&](auto t) {
+          using T = decltype(t);
+          ms_update_xp_kernel<T><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(ms_fields<T>(x, p), vec<T>(r), n / Vec<T>::W, S);
+        });
+      }
+      static void ms_replace_r(const std::vector<ColorSpinorField> &p, ColorSpinorField &r, const ColorSpinorField &r_new, double r2,
+                               const Exec &ex)
+      {
+        size_t n = 0;
+        for (const ColorSpinorField &f : p) n = ms_check(r, f, r_new);
+        double *S = workspace<MsTraits>(ex.stream).scalars;
+        launch(r.precision, 3 * (long long)n * p.size(), [&](auto t) {
+          using T = decltype(t);
+          ms_replace_r_kernel<T><<<kBlocks, kThreads, 0, cs(ex.stream)>>>(ms_fields<T>({}, p), vec<T>(r), vec<T>(r_new), n / Vec<T>::W, S, r2);
+        });
+      }
+      // the device scalar block of Tr as it stands once the stream has drained
+      template <typename Tr> static std::vector<double> fetch(const Exec &ex)
+      {
+        std::vector<double> S(Tr::kCount);
+        cuda_ok(cudaMemcpyAsync(S.data(), workspace<Tr>(ex.stream).scalars, sizeof(double) * Tr::kCount, cudaMemcpyDeviceToHost,
+                                cs(ex.stream)), "memcpy(scalars)");
+        cuda_ok(cudaStreamSynchronize(cs(ex.stream)), "sync");
+        return S;
       }
     } // namespace blas
 
@@ -1254,10 +1524,10 @@ namespace b200
       site(x_other, tmp, other_parity, true);
     }
 
-    // ------------------------------------------------------------------ what CG and BiCGStab share
+    // ------------------------------------------------------------------ what the solvers share
     // Argument checks, the precise work fields r (residual), y (accumulated solution) and tmp, the sloppy solution xS and
     // residual rS (r itself when both operators have one precision), the true residual in the precise operator `op`
-    // (MdagM for CG, M for BiCGStab) and the statistics of SolverParam.
+    // (MdagM for CG and multi-shift CG, M for BiCGStab) plus `shift`, and the statistics of SolverParam.
     namespace
     {
       struct Solve {
@@ -1277,6 +1547,7 @@ namespace b200
         ColorSpinorField &r = r_s.f, &y = y_s.f, &tmp = tmp_s.f, &xS = xS_s.f;
         ColorSpinorField rS;
         double b2 = 0.0;
+        double shift = 0.0; // residual() is taken for op + shift (multi-shift CG; 0 for CG and BiCGStab)
 
         // checks the arguments; returns the sloppy precision
         static int sloppy_precision(const Dirac &mat, const Dirac &matSloppy, const ColorSpinorField &x, const ColorSpinorField &b)
@@ -1301,12 +1572,17 @@ namespace b200
         Scratch sloppy() const { return Scratch(ex.stream, x.X, sp, x.n_parity); }
 
         // b2 = |b|^2; if b == 0, x = 0 and there is nothing to solve
-        bool zero_source(SolverParam &param)
+        bool zero_source()
         {
           b2 = blas::norm2(b, ex);
           syncs++;
           if (b2 != 0.0) return false;
           blas::zero(x, ex);
+          return true;
+        }
+        bool zero_source(SolverParam &param)
+        {
+          if (!zero_source()) return false;
           param.iter = 0;
           param.true_res = 0.0;
           return true;
@@ -1315,6 +1591,7 @@ namespace b200
         double residual(const ColorSpinorField &z)
         {
           (mat.*op)(tmp, z);
+          if (shift != 0.0) blas::axpy(shift, z, tmp, ex);
           blas::copy(r, b, ex);
           const double r2 = blas::axpyNorm(-1.0, tmp, r, ex);
           syncs++;
@@ -1329,16 +1606,17 @@ namespace b200
           blas::zero(xS, ex);
           return r2;
         }
-        // y += xS, staged through tmp when the precisions differ
-        void fold()
+        // acc += sloppy, staged through tmp when the precisions differ
+        void fold(ColorSpinorField &acc, const ColorSpinorField &sloppy)
         {
           if (same_prec) {
-            blas::axpy(1.0, xS, y, ex);
+            blas::axpy(1.0, sloppy, acc, ex);
           } else {
-            blas::copy(tmp, xS, ex);
-            blas::axpy(1.0, tmp, y, ex);
+            blas::copy(tmp, sloppy, ex);
+            blas::axpy(1.0, tmp, acc, ex);
           }
         }
+        void fold() { fold(y, xS); }
         // reliable update: fold the sloppy solution into y, xS = 0, r = b - op y; returns |r|^2
         double reliable_update()
         {
@@ -1352,10 +1630,15 @@ namespace b200
           fold();
           blas::copy(x, y, ex);
           const double tr2 = residual(x);
-          cuda_ok(cudaStreamSynchronize(cs(ex.stream)), "sync");
-          if (halo_timed_out(ex.comm, ex.stream)) throw Error("a halo wait timed out during the solve: the result is not valid");
+          complete(param);
           param.iter = iter;
           param.true_res = std::sqrt(tr2 / b2);
+        }
+        // waits for the solve, checks the halo exchange and fills in the statistics common to every solver
+        template <typename P> void complete(P &param)
+        {
+          cuda_ok(cudaStreamSynchronize(cs(ex.stream)), "sync");
+          if (halo_timed_out(ex.comm, ex.stream)) throw Error("a halo wait timed out during the solve: the result is not valid");
           param.host_syncs = syncs;
           param.secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
           const long long nds = mat.DslashApplications() + matSloppy.DslashApplications() - ds0;
@@ -1538,6 +1821,189 @@ namespace b200
         prev = p4;
       }
       s.finish(param, k);
+    }
+
+    // ------------------------------------------------------------------ multi-shift CG (MdagM + sigma_j) with reliable updates
+    // The CG-M recursion of the reference (lib/inv_multi_cg_quda.cpp): the Krylov space does not depend on the shift, so one
+    // recursion on the smallest shift sigma_0 solves every shift for the operator cost of that one.  With CG's structure:
+    // every scalar lives in one device block (blas::ms_scalars, run by the reduction finalisers), one iteration is
+    // Ap = MdagM p_0, ms_dot, ms_update_r and ms_update_xp, and the host reads |r|^2, the active-shift count and the done
+    // flag of iteration k - 1 while the GPU runs iteration k.  Shifts retire from the top; once all have, the kernels of the
+    // iteration queued behind return at once, so the reported iteration count matches the solution.
+    // Reliable updates (mixed precision) follow shift 0 with CG's criterion, as the reference's do: every x_j takes its
+    // sloppy sum, r = b - (MdagM + sigma_0) x_0 is recomputed in the precise operator, and ms_replace_r repairs p_j with
+    // zeta_j (r_true - r).  The residuals of the other shifts are then taken as zeta_j r_true; the drift that leaves is
+    // what the single-shift refinement in invertMultiShiftCG removes.
+    // More than one shift needs x_j = 0 on entry (collinear residuals); one shift may start from any x_0.
+    static void multishift_cg(const Dirac &mat, const Dirac &matSloppy, std::vector<ColorSpinorField> &x, const ColorSpinorField &b,
+                              MultiShiftParam &param)
+    {
+      using namespace blas;
+      const int n = param.n_shift;
+      Solve s(mat, matSloppy, &Dirac::MdagM, x[0], b);
+      const Exec &ex = s.ex;
+      s.shift = param.offset[0];
+      Scratch Ap_s = s.sloppy();
+      ColorSpinorField &Ap = Ap_s.f, &rS = s.rS;
+      std::deque<Scratch> pool_p, pool_xS;
+      std::vector<ColorSpinorField> p, xS, acc; // per shift: direction, sloppy solution, precise accumulator
+      for (int j = 0; j < n; j++) {
+        p.push_back(pool_p.emplace_back(ex.stream, x[0].X, s.sp, x[0].n_parity).f);
+        xS.push_back(j == 0 ? s.xS : pool_xS.emplace_back(ex.stream, x[0].X, s.sp, x[0].n_parity).f);
+        acc.push_back(j == 0 ? s.y : x[j]);
+      }
+      param.reliable_updates = 0;
+      for (int j = 0; j < n; j++) {
+        param.iter_offset[j] = param.refine_iter[j] = 0;
+        param.iter_res_offset[j] = param.true_res_offset[j] = 0.0;
+      }
+      if (s.zero_source()) {
+        param.iter = 0;
+        s.complete(param);
+        return;
+      }
+
+      double r2 = s.start();
+      Scalars<M_COUNT> s0 {};
+      s0.s[M_R2] = r2;
+      for (int j = 0; j < n; j++) {
+        if (j > 0) zero(xS[j], ex);
+        copy(p[j], rS, ex);
+        s0.s[M_DSIG + j] = param.offset[j] - param.offset[0];
+        s0.s[M_ZETA + j] = s0.s[M_ZOLD + j] = s0.s[M_ALPHA + j] = 1.0;
+        s0.s[M_STOP + j] = param.tol_offset[j] * param.tol_offset[j] * s.b2;
+        s0.s[M_RES + j] = r2;
+        s0.s[M_RETIRED + j] = -1.0;
+      }
+      int n_seen = n; // the active shifts as the host last saw them
+      while (n_seen > 0 && r2 <= s0.s[M_STOP + n_seen - 1]) s0.s[M_RETIRED + --n_seen] = 0.0;
+      s0.s[M_NACT] = n_seen;
+      set_all<MsTraits>(ex, s0);
+      const double stop = s0.s[M_STOP];
+      double rNorm = std::sqrt(r2), r0Norm = rNorm, maxrx = rNorm, maxrr = rNorm;
+      int k = 0;
+
+      // convergence / reliable-update decision on the scalar block after iteration j; true if r was replaced
+      bool done = n_seen == 0;
+      auto decide = [&](const double *S, int j) {
+        r2 = S[M_R2];
+        n_seen = (int)S[M_NACT];
+        const bool converged = S[M_DONE] != 0.0;
+        if (converged) k = j; // the iteration queued after j returned at once
+        rNorm = std::sqrt(r2);
+        if (rNorm > maxrx) maxrx = rNorm;
+        if (rNorm > maxrr) maxrr = rNorm;
+        const bool update = !s.same_prec
+          && ((rNorm < param.delta * maxrx && r0Norm <= maxrx) || (rNorm < param.delta * r0Norm && r0Norm <= maxrr) || converged);
+        if (!update) {
+          done = converged;
+          return false;
+        }
+        // the shifts still active after iteration j take their sloppy sums now; a retired shift keeps its sum until the end
+        for (int i = 1; i < n_seen; i++) {
+          s.fold(acc[i], xS[i]);
+          zero(xS[i], ex);
+        }
+        r2 = s.reliable_update();
+        copy(Ap, s.r, ex); // the true residual in the sloppy precision; Ap is free until the next iteration
+        ms_replace_r(p, rS, Ap, r2, ex);
+        param.reliable_updates++;
+        rNorm = std::sqrt(r2);
+        maxrr = maxrx = r0Norm = rNorm;
+        done = r2 <= stop && n_seen <= 1;
+        return true;
+      };
+
+      Pending prev {};
+      bool have_prev = false;
+      while (!done && k < param.maxiter) {
+        matSloppy.MdagM(Ap, p[0]);
+        ms_dot(p[0], Ap, param.offset[0], ex, s.syncs);
+        Pending pr = ms_update_r(rS, Ap, ex, s.syncs);
+        ms_update_xp(xS, p, rS, std::max(n_seen, 1), ex);
+        k++;
+        if (s.host_ar) { // every reduction has already been waited for
+          decide(await<MsTraits>(pr), k);
+          continue;
+        }
+        bool restarted = false;
+        if (have_prev) {
+          restarted = decide(await<MsTraits>(prev), k - 1);
+          s.syncs++;
+        }
+        // after a restart the pending scalars belong to the recursion before it
+        have_prev = !restarted;
+        prev = pr;
+      }
+
+      // every shift takes its sloppy sum; then the per-shift statistics and true residuals
+      for (int j = 1; j < n; j++) s.fold(acc[j], xS[j]);
+      s.fold();
+      copy(x[0], s.y, ex);
+      const std::vector<double> S = fetch<MsTraits>(ex);
+      s.syncs++;
+      for (int j = 0; j < n; j++) {
+        s.shift = param.offset[j];
+        param.true_res_offset[j] = std::sqrt(s.residual(x[j]) / s.b2);
+        param.iter_res_offset[j] = std::sqrt(S[M_RES + j] / s.b2);
+        param.iter_offset[j] = S[M_RETIRED + j] < 0.0 ? k : (int)S[M_RETIRED + j];
+      }
+      s.complete(param);
+      param.iter = k;
+    }
+
+    void checkMultiShiftParam(const MultiShiftParam &param)
+    {
+      const int n = param.n_shift;
+      if (n < 1 || n > B200_MAX_SHIFTS)
+        throw Error("multi-shift CG: n_shift " + std::to_string(n) + " is outside 1.." + std::to_string(B200_MAX_SHIFTS));
+      for (int j = 0; j < n; j++) {
+        if (!std::isfinite(param.offset[j])) throw Error("multi-shift CG: offset " + std::to_string(j) + " is not finite");
+        if (j > 0 && param.offset[j] < param.offset[j - 1])
+          throw Error("multi-shift CG: the offsets must be non-decreasing (offset " + std::to_string(j) + " is below offset " +
+                      std::to_string(j - 1) + ")");
+        if (!(param.tol_offset[j] > 0.0)) throw Error("multi-shift CG: tol_offset " + std::to_string(j) + " must be > 0");
+      }
+    }
+
+    // The public solve (invertMultiShiftQuda's order): the multi-shift recursion from x_j = 0, then every shift whose true
+    // residual misses its tolerance is refined by the same solver with that single shift, starting from x_j -- which is CG
+    // on MdagM + sigma_j with reliable updates.
+    void invertMultiShiftCG(const Dirac &mat, const Dirac &matSloppy, std::vector<ColorSpinorField> &x, const ColorSpinorField &b,
+                            MultiShiftParam &param)
+    {
+      checkMultiShiftParam(param);
+      const int n = param.n_shift;
+      if ((int)x.size() != n) throw Error("multi-shift CG: " + std::to_string(x.size()) + " solution fields for " + std::to_string(n) + " shifts");
+      for (int j = 0; j < n; j++) {
+        if (x[j].precision != mat.Precision()) throw Error("x and b must have the precise operator's precision");
+        if (x[j].n_parity != b.n_parity || x[j].v == b.v) throw Error("multi-shift CG: each x_j must be a field of b's shape, apart from b");
+        for (int i = 0; i < j; i++)
+          if (x[i].v == x[j].v) throw Error("multi-shift CG: the solution fields must be distinct");
+      }
+      Solve::sloppy_precision(mat, matSloppy, x[0], b);
+      for (ColorSpinorField &f : x) blas::zero(f, mat.exec());
+      multishift_cg(mat, matSloppy, x, b, param);
+      double secs = param.secs, flops = param.gflops * param.secs;
+      for (int j = 0; j < n; j++) {
+        if (!(param.true_res_offset[j] > param.tol_offset[j])) continue;
+        MultiShiftParam one;
+        one.n_shift = 1;
+        one.offset[0] = param.offset[j];
+        one.tol_offset[0] = param.tol_offset[j];
+        one.maxiter = param.maxiter;
+        one.delta = param.delta;
+        std::vector<ColorSpinorField> xj {x[j]};
+        multishift_cg(mat, matSloppy, xj, b, one);
+        param.refine_iter[j] = one.iter;
+        param.true_res_offset[j] = one.true_res_offset[0];
+        param.reliable_updates += one.reliable_updates;
+        param.host_syncs += one.host_syncs;
+        secs += one.secs;
+        flops += one.gflops * one.secs;
+      }
+      param.secs = secs;
+      param.gflops = secs > 0.0 ? flops / secs : 0.0;
     }
 
   } // namespace host

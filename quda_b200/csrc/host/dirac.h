@@ -2,14 +2,15 @@
 // through Dirac::M / MdagM / prepare / reconstruct and invertQuda's CG and BiCGStab.
 //   reference surface   include/dslash_quda.h:83-811 (Apply*), include/dirac_quda.h (Dirac* classes),
 //                       lib/blas_quda.cu + lib/reduce_quda.cu (blas), lib/inv_cg_quda.cpp:63-420 (CG, reliable updates),
-//                       lib/inv_bicgstab_quda.cpp (BiCGStab)
+//                       lib/inv_bicgstab_quda.cpp (BiCGStab), lib/inv_multi_cg_quda.cpp (multi-shift CG)
 // Design (not a mirror of the reference's class tree):
 //   * ONE operator class.  An even-odd operator is described by its site term A (identity, clover, twist) and whether it
 //     is the full matrix or the Schur complement; M / Mdag / prepare / reconstruct are short sequences of two
 //     primitives -- `hop` (a Dslash launch with the site term fused into its epilogue) and `site` (A or A^-1 alone).
 //   * Everything runs on the operator's stream: Dslash, blas, reductions, the NVLink all-reduce.  Reductions are
 //     two-stage and summed in a fixed order (bit-reproducible); their results stay on the device -- each solver's
-//     scalars (CG's alpha, beta; BiCGStab's rho, alpha, omega, beta) are computed there and consumed by the next kernel,
+//     scalars (CG's alpha, beta; BiCGStab's rho, alpha, omega, beta; multi-shift CG's per-shift zeta, alpha, beta) are
+//     computed there and consumed by the next kernel,
 //     the host only follows one iteration behind to decide convergence / reliable updates, so no iteration waits for a
 //     host round trip.
 // Errors throw b200::host::Error (the analogue of errorQuda); everything bottoms out in include/b200_dslash.h.
@@ -227,6 +228,31 @@ namespace b200
     // ---- BiCGStab on M itself (behaviour of lib/inv_bicgstab_quda.cpp): the same precise / sloppy split and SolverParam;
     // restarts after a breakdown are counted in reliable_updates
     void invertBiCGStab(const Dirac &mat, const Dirac &matSloppy, ColorSpinorField &x, const ColorSpinorField &b, SolverParam &param);
+
+    // ---- multi-shift CG on MdagM + sigma_j (behaviour of lib/inv_multi_cg_quda.cpp and the refinement of
+    // invertMultiShiftQuda, lib/interface_quda.cpp:3580-3690)
+    struct MultiShiftParam {
+      int n_shift = 0;
+      double offset[B200_MAX_SHIFTS] = {};     // non-decreasing
+      double tol_offset[B200_MAX_SHIFTS] = {}; // per shift
+      int maxiter = 10000;
+      double delta = 0.1;
+      // results
+      int iter = 0;                              // multi-shift iterations
+      int iter_offset[B200_MAX_SHIFTS] = {};     // iteration at which each shift retired
+      int refine_iter[B200_MAX_SHIFTS] = {};     // iterations of each shift's refinement solve
+      double iter_res_offset[B200_MAX_SHIFTS] = {};
+      double true_res_offset[B200_MAX_SHIFTS] = {};
+      int reliable_updates = 0;
+      double secs = 0.0;
+      double gflops = 0.0;
+      int host_syncs = 0;
+    };
+    // throws unless 1 <= n_shift <= B200_MAX_SHIFTS, the offsets are finite and non-decreasing and every tol_offset > 0
+    void checkMultiShiftParam(const MultiShiftParam &param);
+    // Solve (MdagM + offset[j]) x_j = b for j < n_shift; x holds n_shift fields, which are overwritten
+    void invertMultiShiftCG(const Dirac &mat, const Dirac &matSloppy, std::vector<ColorSpinorField> &x, const ColorSpinorField &b,
+                            MultiShiftParam &param);
 
     // true if a halo wait gave up since the last call (clears the flag); the C entry points turn it into an error
     bool halo_timed_out(CommContext *comm, void *stream);

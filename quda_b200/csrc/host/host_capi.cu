@@ -1,6 +1,8 @@
 // C entry points of the operator / solver layer (declared in include/b200_dslash.h).
 #include <cstring>
 #include <memory>
+#include <string>
+#include <vector>
 
 #include "dirac.h"
 
@@ -183,13 +185,21 @@ int b200_dirac_reconstruct(b200_dirac *h, const b200_spinor *x, const b200_spino
   });
 }
 
+} // extern "C"
+
 using Solver = void (*)(const Dirac &, const Dirac &, ColorSpinorField &, const ColorSpinorField &, SolverParam &);
 
-// argument checks, comm mirroring and parameter marshaling shared by the solver entry points
-static int invert(const char *name, Solver solve, b200_dirac *precise, b200_dirac *sloppy, const b200_spinor *x,
-                  const b200_spinor *b, b200_solver_param *param)
+// argument checks and comm mirroring shared by the solver entry points: `check` refuses a bad parameter block before a
+// device is needed, `solve(precise, sloppy)` runs the solve
+template <typename C, typename F>
+static int invert(const char *name, b200_dirac *precise, b200_dirac *sloppy, const void *param, C &&check, F &&solve)
 {
   if (!precise || !param) return b200::set_error(B200_ERR_INVALID, "%s: null argument", name);
+  try {
+    check();
+  } catch (const Error &e) {
+    return b200::set_error(B200_ERR_INVALID, "%s: %s", name, e.what());
+  }
   if (int rc = b200::require_device()) return rc;
   return guarded([&] {
     if (!sloppy) sloppy = precise;
@@ -200,12 +210,21 @@ static int invert(const char *name, Solver solve, b200_dirac *precise, b200_dira
       if (precise->has_comm != sloppy->has_comm) throw Error("precise / sloppy operators disagree on partitioning");
       pull_comm(sloppy);
     }
-    auto xf = wrap(precise, x), bf = wrap(precise, b);
+    solve(*precise, *sloppy);
+  });
+}
+
+// parameter marshaling of the single-system solvers
+static int invert(const char *name, Solver solve, b200_dirac *precise, b200_dirac *sloppy, const b200_spinor *x,
+                  const b200_spinor *b, b200_solver_param *param)
+{
+  return invert(name, precise, sloppy, param, [] {}, [&](b200_dirac_s &pr, b200_dirac_s &sl) {
+    auto xf = wrap(&pr, x), bf = wrap(&pr, b);
     SolverParam sp;
     sp.tol = param->tol;
     sp.maxiter = param->maxiter;
     sp.delta = param->delta > 0 ? param->delta : 0.1;
-    solve(*precise->op, *sloppy->op, xf, bf, sp);
+    solve(*pr.op, *sl.op, xf, bf, sp);
     param->iter = sp.iter;
     param->reliable_updates = sp.reliable_updates;
     param->true_res = sp.true_res;
@@ -215,6 +234,8 @@ static int invert(const char *name, Solver solve, b200_dirac *precise, b200_dira
   });
 }
 
+extern "C" {
+
 int b200_invert_bicgstab(b200_dirac *precise, b200_dirac *sloppy, const b200_spinor *x, const b200_spinor *b, b200_solver_param *param)
 {
   return invert("b200_invert_bicgstab", invertBiCGStab, precise, sloppy, x, b, param);
@@ -223,5 +244,40 @@ int b200_invert_bicgstab(b200_dirac *precise, b200_dirac *sloppy, const b200_spi
 int b200_invert_cg(b200_dirac *precise, b200_dirac *sloppy, const b200_spinor *x, const b200_spinor *b, b200_solver_param *param)
 {
   return invert("b200_invert_cg", invertCG, precise, sloppy, x, b, param);
+}
+
+int b200_invert_multishift_cg(b200_dirac *precise, b200_dirac *sloppy, const b200_spinor *x, const b200_spinor *b,
+                              b200_multishift_param *param)
+{
+  MultiShiftParam mp;
+  auto check = [&] {
+    mp.n_shift = param->n_shift;
+    memcpy(mp.offset, param->offset, sizeof(mp.offset));
+    memcpy(mp.tol_offset, param->tol_offset, sizeof(mp.tol_offset));
+    mp.maxiter = param->maxiter;
+    mp.delta = param->delta > 0 ? param->delta : 0.1;
+    checkMultiShiftParam(mp);
+    if (!x || !b) throw Error("null spinor");
+    for (int j = 0; j < mp.n_shift; j++)
+      if (!x[j].v) throw Error("solution descriptor " + std::to_string(j) + " has no field");
+  };
+  return invert("b200_invert_multishift_cg", precise, sloppy, param, check, [&](b200_dirac_s &pr, b200_dirac_s &sl) {
+    std::vector<ColorSpinorField> xs;
+    for (int j = 0; j < mp.n_shift; j++) xs.push_back(wrap(&pr, &x[j]));
+    auto bf = wrap(&pr, b);
+    invertMultiShiftCG(*pr.op, *sl.op, xs, bf, mp);
+    param->iter = mp.iter;
+    for (int j = 0; j < B200_MAX_SHIFTS; j++) {
+      const bool on = j < mp.n_shift;
+      param->iter_offset[j] = on ? mp.iter_offset[j] : 0;
+      param->refine_iter[j] = on ? mp.refine_iter[j] : 0;
+      param->iter_res_offset[j] = on ? mp.iter_res_offset[j] : 0.0;
+      param->true_res_offset[j] = on ? mp.true_res_offset[j] : 0.0;
+    }
+    param->reliable_updates = mp.reliable_updates;
+    param->secs = mp.secs;
+    param->gflops = mp.gflops;
+    param->host_syncs = mp.host_syncs;
+  });
 }
 }

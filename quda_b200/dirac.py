@@ -1,8 +1,9 @@
 """Thin Python handles on the C++ operator / solver layer (quda_b200/csrc/host/dirac.h): DiracWilson[PC],
 DiracClover[PC], DiracTwistedMass[PC] (reference: lib/dirac_wilson.cpp, lib/dirac_clover.cpp, lib/dirac_twisted_mass.cpp),
-CG on the normal equations (lib/inv_cg_quda.cpp) and BiCGStab on M itself (lib/inv_bicgstab_quda.cpp), both mixed-precision
-with reliable updates.  All arithmetic happens in libquda_b200.so; this module only marshals descriptors."""
+CG on the normal equations (lib/inv_cg_quda.cpp), BiCGStab on M itself (lib/inv_bicgstab_quda.cpp) and multi-shift CG on
+MdagM + sigma_j (lib/inv_multi_cg_quda.cpp), all mixed-precision with reliable updates.  All arithmetic happens in libquda_b200.so; this module only marshals descriptors."""
 import ctypes as C
+import math
 
 from . import lib as L
 
@@ -92,3 +93,35 @@ def invert_cg(precise, sloppy, x, b, tol=1e-10, maxiter=10000, delta=0.1):
 def invert_bicgstab(precise, sloppy, x, b, tol=1e-10, maxiter=10000, delta=0.1):
     """BiCGStab on M x = b with the operator as given (lib/inv_bicgstab_quda.cpp)."""
     return _invert("invert_bicgstab", precise, sloppy, x, b, tol, maxiter, delta)
+
+
+def invert_multishift_cg(precise, sloppy, xs, b, offsets, tol=1e-10, tol_offset=None, maxiter=10000, delta=0.1):
+    """Multi-shift CG: (MdagM + offsets[j]) xs[j] = b for every shift at once (lib/inv_multi_cg_quda.cpp, with the refinement
+    of invertMultiShiftQuda).  The operator is taken as given (the Schur complement for the *pc types).  offsets must be
+    finite and non-decreasing; tol_offset (default: tol for every shift) gives each shift its own target.  Every xs[j] is
+    overwritten.  Returns the filled MultiShiftParam (iter, iter_offset, refine_iter, iter_res_offset, true_res_offset,
+    reliable_updates, secs, gflops, host_syncs)."""
+    name = "invert_multishift_cg"
+    offsets = [float(o) for o in offsets]
+    n = len(offsets)
+    if not 1 <= n <= L.MAX_SHIFTS:
+        raise L.B200Error(f"{name}: {n} offsets, between 1 and {L.MAX_SHIFTS} are supported")
+    if not all(math.isfinite(o) for o in offsets) or any(hi < lo for lo, hi in zip(offsets, offsets[1:])):
+        raise L.B200Error(f"{name}: the offsets must be finite and non-decreasing, got {offsets}")
+    tols = [float(tol)] * n if tol_offset is None else [float(t) for t in tol_offset]
+    if len(tols) != n or not all(t > 0 for t in tols):
+        raise L.B200Error(f"{name}: tol_offset needs one positive tolerance per offset, got {tols}")
+    if len(xs) != n:
+        raise L.B200Error(f"{name}: {len(xs)} solution fields for {n} offsets")
+    for what, f in [(f"x[{j}]", x) for j, x in enumerate(xs)] + [("b", b)]:
+        if f.prec != precise.prec:
+            raise L.B200Error(f"{name}: {what} has precision {f.prec}, the precise operator {precise.prec}")
+    p = L.MultiShiftParam()
+    p.n_shift, p.maxiter, p.delta = n, maxiter, delta
+    for j in range(n):
+        p.offset[j], p.tol_offset[j] = offsets[j], tols[j]
+    xd = (L.Spinor * n)(*[x.desc() for x in xs])
+    bd = b.desc()
+    L.check(precise.lib.b200_invert_multishift_cg(precise.h, sloppy.h if sloppy is not None else None, xd, C.byref(bd),
+                                                  C.byref(p)))
+    return p

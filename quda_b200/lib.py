@@ -78,6 +78,17 @@ class SolverParam(C.Structure):
                 ("host_syncs", C.c_int)]
 
 
+MAX_SHIFTS = 32
+
+
+class MultiShiftParam(C.Structure):
+    _fields_ = [("n_shift", C.c_int), ("offset", C.c_double * MAX_SHIFTS), ("tol_offset", C.c_double * MAX_SHIFTS),
+                ("maxiter", C.c_int), ("delta", C.c_double), ("iter", C.c_int), ("iter_offset", C.c_int * MAX_SHIFTS),
+                ("refine_iter", C.c_int * MAX_SHIFTS), ("iter_res_offset", C.c_double * MAX_SHIFTS),
+                ("true_res_offset", C.c_double * MAX_SHIFTS), ("reliable_updates", C.c_int), ("secs", C.c_double),
+                ("gflops", C.c_double), ("host_syncs", C.c_int)]
+
+
 MAX_MULTI_RHS = 16
 DIRAC_WILSON, DIRAC_WILSONPC, DIRAC_CLOVER, DIRAC_CLOVERPC, DIRAC_TWISTED_MASS, DIRAC_TWISTED_MASSPC = 0, 1, 2, 3, 4, 5
 APPLY_M, APPLY_MDAG, APPLY_MDAGM, APPLY_DSLASH, APPLY_DSLASH_XPAY = 0, 1, 2, 3, 4
@@ -154,6 +165,9 @@ def load():
         lib.b200_invert_cg.restype = C.c_int
         lib.b200_invert_bicgstab.argtypes = lib.b200_invert_cg.argtypes
         lib.b200_invert_bicgstab.restype = C.c_int
+        lib.b200_invert_multishift_cg.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(Spinor), C.POINTER(Spinor),
+                                                  C.POINTER(MultiShiftParam)]
+        lib.b200_invert_multishift_cg.restype = C.c_int
         lib.b200_comm_check.argtypes, lib.b200_comm_check.restype = [C.POINTER(Comm), C.c_void_p], C.c_int
         if lib.b200_abi_version() != ABI_VERSION:
             raise B200Error("libquda_b200.so ABI version mismatch")
@@ -172,5 +186,6 @@ EXPORTED_SYMBOLS = ["b200_dslash_apply", "b200_dslash_apply_fused", "b200_dslash
                     "b200_copy_spinor", "b200_copy_gauge", "b200_copy_clover", "b200_comm_alloc", "b200_comm_free", "b200_ipc_get_handle", "b200_ipc_open_handle",
                     "b200_ipc_close_handle", "b200_comm_copy",
                     "b200_dirac_create", "b200_dirac_set_twist", "b200_dirac_destroy", "b200_dirac_apply", "b200_dirac_prepare",
-                    "b200_dirac_reconstruct", "b200_invert_cg", "b200_invert_bicgstab", "b200_comm_check",
+                    "b200_dirac_reconstruct", "b200_invert_cg", "b200_invert_bicgstab", "b200_invert_multishift_cg",
+                    "b200_comm_check",
                     "b200_last_error", "b200_abi_version", "b200_launch_count", "b200_reset_launch_count"]
