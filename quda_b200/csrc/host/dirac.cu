@@ -2,7 +2,6 @@
 #include <algorithm>
 #include <chrono>
 #include <cmath>
-#include <cstdio>
 #include <cstdlib>
 #include <cstdint>
 #include <cstring>
@@ -448,14 +447,25 @@ namespace b200
       // Second stage of every reduction, run by the block that arrives last: sum the per-block partial sums in block
       // order (fixed -> bit-reproducible), all-reduce over the ranks through the NVLink mailboxes in rank order, store the
       // global sums in the raw slots, derive the solver's scalars and publish the scalar block to the host mirror.
-      template <int NV, typename Tr>
-      __device__ void finish_reduction(const double *acc_block, double *partials, unsigned *ticket, double *S, double *host_out,
-                                       int fin, ReducePeers peers)
+      struct ReduceArgs {
+        double *partials; // [kBlocks][Tr::kVals]
+        unsigned *ticket;
+        double *S;        // the solver's scalar block
+        double *host_out; // its mirror slot, or null
+        int fin;          // the finaliser: what Tr::derive computes from the sums
+        ReducePeers peers;
+      };
+      template <int NV, typename Tr> __device__ void finish_reduction(const double *acc_block, const ReduceArgs &ra)
       {
         constexpr int MV = Tr::kVals;
         __shared__ double sh[kThreads][MV];
         __shared__ bool is_last;
         __shared__ double part[B200_MAX_RANKS][MV];
+        // copies of the arguments: reading them in place, peers above all, gives the finalisers another schedule
+        double *partials = ra.partials, *S = ra.S, *host_out = ra.host_out;
+        unsigned *ticket = ra.ticket;
+        const int fin = ra.fin;
+        const ReducePeers peers = ra.peers;
         const int t = threadIdx.x;
         if (t == 0) {
           for (int i = 0; i < NV; i++) partials[blockIdx.x * MV + i] = acc_block[i];
@@ -534,15 +544,15 @@ namespace b200
         __syncthreads();
         return s;
       }
-
-      struct ReduceArgs {
-        double *partials;
-        unsigned *ticket;
-        double *S;
-        double *host_out;
-        int fin;
-        ReducePeers peers;
-      };
+      // the tail of every reduction kernel: the block sum of each per-thread value, then the second stage
+      template <typename Tr, int NV> __device__ __forceinline__ void reduce_block(const double (&acc)[NV], const ReduceArgs &ra)
+      {
+        __shared__ double wb[kThreads / 32];
+        double s[NV];
+#pragma unroll
+        for (int i = 0; i < NV; i++) s[i] = block_sum(acc[i], wb);
+        finish_reduction<NV, Tr>(s, ra);
+      }
 
       // y = a x + b y with an optional reduction over the result (R_NORM_Y) or <x, y> (R_DOT_XY)
       enum { R_NONE = 0, R_NORM_Y = 1, R_DOT_XY = 2 };
@@ -558,11 +568,7 @@ namespace b200
           if (R == R_NORM_Y) acc += (write ? (double)(Ty)r * (double)(Ty)r : yv * yv);
           if (R == R_DOT_XY) acc += xv * yv;
         }
-        if (R != R_NONE) {
-          __shared__ double wb[kThreads / 32];
-          const double s = block_sum(acc, wb);
-          finish_reduction<1, CgTraits>(&s, ra.partials, ra.ticket, ra.S, ra.host_out, ra.fin, ra.peers);
-        }
+        if (R != R_NONE) reduce_block<CgTraits>({acc}, ra);
       }
 
       // ---- the three kernels of a CG iteration; alpha and beta come from the device scalars
@@ -577,9 +583,7 @@ namespace b200
           r[i] = v;
           acc += (double)v * (double)v;
         }
-        __shared__ double wb[kThreads / 32];
-        const double s = block_sum(acc, wb);
-        finish_reduction<1, CgTraits>(&s, ra.partials, ra.ticket, ra.S, ra.host_out, ra.fin, ra.peers);
+        reduce_block<CgTraits>({acc}, ra);
       }
       // x += alpha p ; p = r + beta p   (the reference's axpyZpbx, lib/inv_cg_quda.cpp:389)
       template <typename T>
@@ -695,14 +699,6 @@ namespace b200
       // The five streaming kernels of a BiCGStab iteration walk the field as complex numbers: in both native orders (fp64
       // planes of 2 reals, fp32 planes of 4) the real index 2c + re/im keeps each pair adjacent, so element pair i is one
       // complex component.  n is the number of complex elements.  Every kernel returns at once when S[B_DONE] is set.
-      template <int NV> __device__ __forceinline__ void bicg_finish(const double (&acc)[NV], const ReduceArgs &ra)
-      {
-        __shared__ double wb[kThreads / 32];
-        double s[NV];
-#pragma unroll
-        for (int i = 0; i < NV; i++) s[i] = block_sum(acc[i], wb);
-        finish_reduction<NV, BicgTraits>(s, ra.partials, ra.ticket, ra.S, ra.host_out, ra.fin, ra.peers);
-      }
 
       // K1 (and the rho (re)computation): <a, b> = sum conj(a) b
       template <typename T>
@@ -717,7 +713,7 @@ namespace b200
           acc[0] += (double)x.x * y.x + (double)x.y * y.y;
           acc[1] += (double)x.x * y.y - (double)x.y * y.x;
         }
-        bicg_finish<2>(acc, ra);
+        reduce_block<BicgTraits>(acc, ra);
       }
       // K2: s = r - alpha v, in place in r
       template <typename T>
@@ -751,7 +747,7 @@ namespace b200
           acc[2] += (double)x.x * x.x + (double)x.y * x.y;
           acc[3] += (double)y.x * y.x + (double)y.y * y.y;
         }
-        bicg_finish<4>(acc, ra);
+        reduce_block<BicgTraits>(acc, ra);
       }
       // K4: x += alpha p + omega s ; r = s - omega t (r holds s) ; <r0, r>, |r|^2 of the stored r
       template <typename T>
@@ -778,7 +774,7 @@ namespace b200
           acc[1] += (double)hv.x * ro.y - (double)hv.y * ro.x;
           acc[2] += (double)ro.x * ro.x + (double)ro.y * ro.y;
         }
-        bicg_finish<3>(acc, ra);
+        reduce_block<BicgTraits>(acc, ra);
       }
       // K5: p = r + beta (p - omega v)
       template <typename T>
@@ -893,12 +889,6 @@ namespace b200
         T *x[kShifts];
         T *p[kShifts];
       };
-      __device__ __forceinline__ void ms_finish(double acc, const ReduceArgs &ra)
-      {
-        __shared__ double wb[kThreads / 32];
-        const double s = block_sum(acc, wb);
-        finish_reduction<1, MsTraits>(&s, ra.partials, ra.ticket, ra.S, ra.host_out, ra.fin, ra.peers);
-      }
       // Ap += sigma_0 p ; <p, Ap>   (finaliser FIN_PAP).  Once M_DONE is set it returns at once, and clears M_NUPD so
       // that the x / p update queued behind it does nothing either.
       template <typename T>
@@ -920,7 +910,7 @@ namespace b200
           }
           if (sigma != 0.0) Ap[i] = av;
         }
-        ms_finish(acc, ra);
+        reduce_block<MsTraits>({acc}, ra);
       }
       // r -= alpha_0 Ap ; |r|^2   (finaliser FIN_R2: beta_j, retirement, done flag)
       template <typename T>
@@ -940,7 +930,7 @@ namespace b200
           }
           r[i] = rv;
         }
-        ms_finish(acc, ra);
+        reduce_block<MsTraits>({acc}, ra);
       }
       // The hot path: for every shift j < M_NUPD, x_j += alpha_j p_j ; p_j = zeta_j r + beta_j p_j (shift 0: zeta = 1, the
       // reference's axpyZpbx; the others its axpyBzpcx).  r is read once per element; a retired shift costs no bytes:
@@ -1542,6 +1532,8 @@ namespace b200
         const int sp;
         const bool same_prec, host_ar;
         int syncs = 0;
+        int k = 0;         // iterations run
+        bool done = false; // set by the solver's decision
         Scratch r_s, y_s, tmp_s, xS_s;
         std::unique_ptr<Scratch> rS_s;
         ColorSpinorField &r = r_s.f, &y = y_s.f, &tmp = tmp_s.f, &xS = xS_s.f;
@@ -1624,14 +1616,39 @@ namespace b200
           blas::zero(xS, ex);
           return residual(y);
         }
+        // The iteration loop of every solver.  step() queues one iteration and returns the reduction whose scalar block
+        // (of Tr) the host decides on; decide(S, j) reads that block as of iteration j and returns true if it replaced
+        // the residual.  No iteration waits for the host: while the GPU runs iteration k the host decides on k - 1.  With
+        // the host-callback all-reduce every reduction has already been waited for, so it decides on k at once.
+        template <typename Tr, typename Step, typename Decide> void iterate(int maxiter, Step &&step, Decide &&decide)
+        {
+          blas::Pending prev {};
+          bool have_prev = false;
+          while (!done && k < maxiter) {
+            const blas::Pending pend = step();
+            k++;
+            if (host_ar) {
+              decide(blas::await<Tr>(pend), k);
+              continue;
+            }
+            bool replaced = false;
+            if (have_prev) {
+              replaced = decide(blas::await<Tr>(prev), k - 1);
+              syncs++;
+            }
+            // after a replacement the pending scalars belong to the recursion before it
+            have_prev = !replaced;
+            prev = pend;
+          }
+        }
         // x = y + xS, its true residual, and the statistics
-        void finish(SolverParam &param, int iter)
+        void finish(SolverParam &param)
         {
           fold();
           blas::copy(x, y, ex);
           const double tr2 = residual(x);
           complete(param);
-          param.iter = iter;
+          param.iter = k;
           param.true_res = std::sqrt(tr2 / b2);
         }
         // waits for the solve, checks the halo exchange and fills in the statistics common to every solver
@@ -1645,6 +1662,23 @@ namespace b200
           const double fl = (double)(blas::flops() - flops0) + (double)nds * 1320.0 * x.VolumeCB();
           param.gflops = fl / param.secs * 1e-9;
         }
+      };
+
+      // The reliable-update rule of the reference's CG (lib/inv_cg_quda.cpp), shared by CG and multi-shift CG: |r| is
+      // measured against its value r0Norm after the last update and against its maxima since then.
+      struct CgReliable {
+        double r0Norm, maxrx, maxrr;
+        explicit CgReliable(double r2) { reset(r2); }
+        // tracks the maxima; true if |r|^2 = r2 calls for an update (in mixed precision always once converged)
+        bool update(double r2, double delta, bool mixed, bool converged)
+        {
+          const double rNorm = std::sqrt(r2);
+          if (rNorm > maxrx) maxrx = rNorm;
+          if (rNorm > maxrr) maxrr = rNorm;
+          return mixed && ((rNorm < delta * maxrx && r0Norm <= maxrx) || (rNorm < delta * r0Norm && r0Norm <= maxrr) || converged);
+        }
+        // after an update that left |r|^2 = r2
+        void reset(double r2) { r0Norm = maxrx = maxrr = std::sqrt(r2); }
       };
     } // namespace
 
@@ -1667,61 +1701,35 @@ namespace b200
       copy(p, rS, ex);
       set_scalar<CgTraits>(ex, S_R2, r2);
       const double stop = param.tol * param.tol * s.b2;
-      double rNorm = std::sqrt(r2), r0Norm = rNorm, maxrx = rNorm, maxrr = rNorm;
-      int k = 0;
+      CgReliable rel(r2);
       param.reliable_updates = 0;
-      const bool verbose = getenv("B200_CG_VERBOSE") != nullptr;
-      if (verbose) fprintf(stderr, "[cg] b2=%g r2=%g stop=%g mixed=%d\n", s.b2, r2, stop, (int)(&mat != &matSloppy));
 
-      // convergence / reliable-update decision on a residual norm; returns true if the recursion was restarted
-      bool done = false;
-      auto decide = [&](double r2_seen) {
-        rNorm = std::sqrt(r2_seen);
-        if (rNorm > maxrx) maxrx = rNorm;
-        if (rNorm > maxrr) maxrr = rNorm;
-        const bool converged = r2_seen <= stop;
-        const bool update = !s.same_prec
-          && ((rNorm < param.delta * maxrx && r0Norm <= maxrx) || (rNorm < param.delta * r0Norm && r0Norm <= maxrr) || converged);
-        if (verbose && (k < 10 || k % 20 == 0 || update)) fprintf(stderr, "[cg] k=%d r2=%g update=%d\n", k, r2_seen, (int)update);
-        if (update) {
-          // the true residual repairs the recursion: p += r_true - rS ; rS = r_true
-          r2 = s.reliable_update();
-          copy(Ap, s.r, ex); // the true residual in the sloppy precision; Ap is free until the next iteration
-          cg_replace_r(p, rS, Ap, ex);
-          set_scalar<CgTraits>(ex, S_R2, r2);
-          param.reliable_updates++;
-          rNorm = std::sqrt(r2);
-          maxrr = maxrx = r0Norm = rNorm;
-          if (r2 <= stop) done = true;
-          return true;
+      // convergence / reliable-update decision on the scalar block after an iteration (CG has no done flag, so the
+      // iteration queued behind it runs and counts); true if the recursion was restarted
+      auto decide = [&](const double *S, int) {
+        const bool converged = S[S_R2] <= stop;
+        if (!rel.update(S[S_R2], param.delta, !s.same_prec, converged)) {
+          s.done = converged;
+          return false;
         }
-        if (converged) done = true;
-        return false;
+        // the true residual repairs the recursion: p += r_true - rS ; rS = r_true
+        r2 = s.reliable_update();
+        copy(Ap, s.r, ex); // the true residual in the sloppy precision; Ap is free until the next iteration
+        cg_replace_r(p, rS, Ap, ex);
+        set_scalar<CgTraits>(ex, S_R2, r2);
+        param.reliable_updates++;
+        rel.reset(r2);
+        s.done = r2 <= stop;
+        return true;
       };
-
-      Pending prev {};
-      bool have_prev = false;
-      while (!done && k < param.maxiter) {
+      s.iterate<CgTraits>(param.maxiter, [&] {
         matSloppy.MdagM(Ap, p);
         cg_dot(p, Ap, ex, s.syncs);
-        Pending pr = cg_update_r(rS, Ap, ex, s.syncs);
+        const Pending pr = cg_update_r(rS, Ap, ex, s.syncs);
         cg_update_xp(s.xS, p, rS, ex);
-        k++;
-        if (s.host_ar) { // every reduction has already been waited for
-          decide(await<CgTraits>(pr)[S_R2]);
-          continue;
-        }
-        // the host follows one iteration behind: while the GPU runs iteration k it looks at the residual of k - 1
-        bool restarted = false;
-        if (have_prev) {
-          restarted = decide(await<CgTraits>(prev)[S_R2]);
-          s.syncs++;
-        }
-        // after a restart the pending residual belongs to the recursion before it
-        have_prev = !restarted;
-        prev = pr;
-      }
-      s.finish(param, k);
+        return pr;
+      }, decide);
+      s.finish(param);
     }
 
     // ------------------------------------------------------------------ BiCGStab (M x = b) with reliable updates
@@ -1747,7 +1755,6 @@ namespace b200
       if (s.zero_source(param)) return;
       const double stop = param.tol * param.tol * s.b2;
       double r2 = 0.0, maxrr = 0.0;
-      int k = 0;
       param.reliable_updates = 0;
 
       // reliable update in the precise operator, then rS = r; clears the device flags
@@ -1771,13 +1778,13 @@ namespace b200
       s0.s[B_STOP] = stop;
       set_all<BicgTraits>(ex, s0);
       recompute_rho();
-      bool done = r2 <= stop;
+      s.done = r2 <= stop;
 
       // convergence / reliable-update / restart decision on the scalar block after iteration j; true if r was replaced
       auto decide = [&](const double *S, int j) {
         r2 = S[B_R2];
         const bool converged = S[B_DONE] != 0.0, broke = S[B_BREAK] != 0.0;
-        if (converged) k = j; // the iteration queued after j returned at once
+        if (converged) s.k = j; // the iteration queued after j returned at once
         const double rNorm = std::sqrt(r2);
         if (rNorm > maxrr) maxrr = rNorm;
         if (broke) { // restart from the true residual with a new shadow residual
@@ -1787,40 +1794,25 @@ namespace b200
         } else if (!s.same_prec && (converged || rNorm < param.delta * maxrr)) {
           true_residual(); // reliable update: p is kept
         } else {
-          done = converged;
+          s.done = converged;
           return false;
         }
         recompute_rho();
         param.reliable_updates++;
-        done = r2 <= stop;
+        s.done = r2 <= stop;
         return true;
       };
-
-      Pending prev {};
-      bool have_prev = false;
-      while (!done && k < param.maxiter) {
+      s.iterate<BicgTraits>(param.maxiter, [&] {
         matSloppy.M(v, p);
-        bicg_cdot(r0, v, BF_ALPHA, ex, s.syncs);                      // K1
-        bicg_update_s(rS, v, ex);                                      // K2
+        bicg_cdot(r0, v, BF_ALPHA, ex, s.syncs);                            // K1
+        bicg_update_s(rS, v, ex);                                            // K2
         matSloppy.M(t, rS);
-        bicg_ts(t, rS, ex, s.syncs);                                   // K3
-        Pending p4 = bicg_update_xr(s.xS, rS, p, t, r0, ex, s.syncs); // K4
-        bicg_update_p(p, rS, v, ex);                                   // K5
-        k++;
-        if (s.host_ar) { // every reduction has already been waited for
-          decide(await<BicgTraits>(p4), k);
-          continue;
-        }
-        bool replaced = false;
-        if (have_prev) {
-          replaced = decide(await<BicgTraits>(prev), k - 1);
-          s.syncs++;
-        }
-        // after a replacement the pending scalars belong to the recursion before it
-        have_prev = !replaced;
-        prev = p4;
-      }
-      s.finish(param, k);
+        bicg_ts(t, rS, ex, s.syncs);                                         // K3
+        const Pending p4 = bicg_update_xr(s.xS, rS, p, t, r0, ex, s.syncs); // K4
+        bicg_update_p(p, rS, v, ex);                                         // K5
+        return p4;
+      }, decide);
+      s.finish(param);
     }
 
     // ------------------------------------------------------------------ multi-shift CG (MdagM + sigma_j) with reliable updates
@@ -1880,23 +1872,17 @@ namespace b200
       s0.s[M_NACT] = n_seen;
       set_all<MsTraits>(ex, s0);
       const double stop = s0.s[M_STOP];
-      double rNorm = std::sqrt(r2), r0Norm = rNorm, maxrx = rNorm, maxrr = rNorm;
-      int k = 0;
+      CgReliable rel(r2);
+      s.done = n_seen == 0;
 
       // convergence / reliable-update decision on the scalar block after iteration j; true if r was replaced
-      bool done = n_seen == 0;
       auto decide = [&](const double *S, int j) {
         r2 = S[M_R2];
         n_seen = (int)S[M_NACT];
         const bool converged = S[M_DONE] != 0.0;
-        if (converged) k = j; // the iteration queued after j returned at once
-        rNorm = std::sqrt(r2);
-        if (rNorm > maxrx) maxrx = rNorm;
-        if (rNorm > maxrr) maxrr = rNorm;
-        const bool update = !s.same_prec
-          && ((rNorm < param.delta * maxrx && r0Norm <= maxrx) || (rNorm < param.delta * r0Norm && r0Norm <= maxrr) || converged);
-        if (!update) {
-          done = converged;
+        if (converged) s.k = j; // the iteration queued after j returned at once
+        if (!rel.update(r2, param.delta, !s.same_prec, converged)) {
+          s.done = converged;
           return false;
         }
         // the shifts still active after iteration j take their sloppy sums now; a retired shift keeps its sum until the end
@@ -1908,33 +1894,17 @@ namespace b200
         copy(Ap, s.r, ex); // the true residual in the sloppy precision; Ap is free until the next iteration
         ms_replace_r(p, rS, Ap, r2, ex);
         param.reliable_updates++;
-        rNorm = std::sqrt(r2);
-        maxrr = maxrx = r0Norm = rNorm;
-        done = r2 <= stop && n_seen <= 1;
+        rel.reset(r2);
+        s.done = r2 <= stop && n_seen <= 1;
         return true;
       };
-
-      Pending prev {};
-      bool have_prev = false;
-      while (!done && k < param.maxiter) {
+      s.iterate<MsTraits>(param.maxiter, [&] {
         matSloppy.MdagM(Ap, p[0]);
         ms_dot(p[0], Ap, param.offset[0], ex, s.syncs);
-        Pending pr = ms_update_r(rS, Ap, ex, s.syncs);
+        const Pending pr = ms_update_r(rS, Ap, ex, s.syncs);
         ms_update_xp(xS, p, rS, std::max(n_seen, 1), ex);
-        k++;
-        if (s.host_ar) { // every reduction has already been waited for
-          decide(await<MsTraits>(pr), k);
-          continue;
-        }
-        bool restarted = false;
-        if (have_prev) {
-          restarted = decide(await<MsTraits>(prev), k - 1);
-          s.syncs++;
-        }
-        // after a restart the pending scalars belong to the recursion before it
-        have_prev = !restarted;
-        prev = pr;
-      }
+        return pr;
+      }, decide);
 
       // every shift takes its sloppy sum; then the per-shift statistics and true residuals
       for (int j = 1; j < n; j++) s.fold(acc[j], xS[j]);
@@ -1946,10 +1916,10 @@ namespace b200
         s.shift = param.offset[j];
         param.true_res_offset[j] = std::sqrt(s.residual(x[j]) / s.b2);
         param.iter_res_offset[j] = std::sqrt(S[M_RES + j] / s.b2);
-        param.iter_offset[j] = S[M_RETIRED + j] < 0.0 ? k : (int)S[M_RETIRED + j];
+        param.iter_offset[j] = S[M_RETIRED + j] < 0.0 ? s.k : (int)S[M_RETIRED + j];
       }
       s.complete(param);
-      param.iter = k;
+      param.iter = s.k;
     }
 
     void checkMultiShiftParam(const MultiShiftParam &param)

@@ -71,12 +71,17 @@ class Dirac:
         L.check(self.lib.b200_dirac_reconstruct(self.h, C.byref(xd), C.byref(bd)))
 
 
-def _invert(name, precise, sloppy, x, b, tol, maxiter, delta):
-    """Run the C ABI solver b200_<name>; returns the filled SolverParam (iter, true_res, secs, gflops, reliable_updates,
-    host_syncs).  x and b must have the precise operator's precision: the C ABI reads them in that precision."""
-    for what, f in (("x", x), ("b", b)):
+def _need_precise(name, precise, fields):
+    """The C ABI reads the solution and source fields in the precise operator's precision: refuse any other."""
+    for what, f in fields:
         if f.prec != precise.prec:
             raise L.B200Error(f"{name}: {what} has precision {f.prec}, the precise operator {precise.prec}")
+
+
+def _invert(name, precise, sloppy, x, b, tol, maxiter, delta):
+    """Run the C ABI solver b200_<name>; returns the filled SolverParam (iter, true_res, secs, gflops, reliable_updates,
+    host_syncs)."""
+    _need_precise(name, precise, [("x", x), ("b", b)])
     p = L.SolverParam()
     p.tol, p.maxiter, p.delta = tol, maxiter, delta
     xd, bd = x.desc(), b.desc()
@@ -113,9 +118,7 @@ def invert_multishift_cg(precise, sloppy, xs, b, offsets, tol=1e-10, tol_offset=
         raise L.B200Error(f"{name}: tol_offset needs one positive tolerance per offset, got {tols}")
     if len(xs) != n:
         raise L.B200Error(f"{name}: {len(xs)} solution fields for {n} offsets")
-    for what, f in [(f"x[{j}]", x) for j, x in enumerate(xs)] + [("b", b)]:
-        if f.prec != precise.prec:
-            raise L.B200Error(f"{name}: {what} has precision {f.prec}, the precise operator {precise.prec}")
+    _need_precise(name, precise, [(f"x[{j}]", x) for j, x in enumerate(xs)] + [("b", b)])
     p = L.MultiShiftParam()
     p.n_shift, p.maxiter, p.delta = n, maxiter, delta
     for j in range(n):
