@@ -1,26 +1,9 @@
 """CPU tier, world_size = 2 over gloo: process-grid topology, local slicing of global fields, face packing,
 neighbour exchange and the interior + exterior split -- each rank computes its half of a global lattice with
 the host twin and the gathered result must match the oracle on the GLOBAL lattice."""
-import os
-import socket
-import sys
-
-import numpy as np
 import pytest
-import torch.multiprocessing as mp
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-from dist_worker import worker as _worker
+from dist_worker import run_ranks, worker
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -33,37 +16,19 @@ def _twin_built():
 @pytest.mark.parametrize("grid_dims,Xl", [((1, 1, 1, 2), (4, 4, 4, 4)), ((2, 1, 1, 1), (4, 4, 6, 4)), ((1, 2, 1, 1), (4, 4, 4, 6))])
 @pytest.mark.parametrize("prec,recon", [(8, 18), (4, 12), (2, 8)])
 def test_two_rank_wilson_matches_global_oracle(grid_dims, Xl, prec, recon):
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, 2, port, grid_dims, Xl, prec, recon, q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = [q.get(timeout=300) for _ in procs]
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    res = run_ranks(worker, 2, (grid_dims, Xl, prec, recon), timeout=300)
     tol = {8: 1e-11, 4: 1e-4, 2: 1e-2}[prec]
-    for rank, dev, _ in res:
-        assert dev <= tol, (rank, dev)
+    for r in res:
+        assert r["dev"] <= tol, (r["rank"], r["dev"])
 
 
 @pytest.mark.parametrize("grid_dims,Xl,prec,recon", [((1, 1, 1, 2), (4, 4, 4, 4), 8, 18), ((2, 1, 1, 1), (4, 4, 6, 4), 2, 12)])
 def test_two_rank_batched_halo_matches_global_oracle(grid_dims, Xl, prec, recon):
     """a multi-RHS batch on a partitioned lattice: one batched exchange for 3 sources (HaloExchange(n_src=3))"""
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, 2, port, grid_dims, Xl, prec, recon, q, "host", 2, 3)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = [q.get(timeout=300) for _ in procs]
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    res = run_ranks(worker, 2, (grid_dims, Xl, prec, recon, "host", 2, 3), timeout=300)
     tol = {8: 1e-11, 4: 1e-4, 2: 1e-2}[prec]
-    for rank, dev, _ in res:
-        assert dev <= tol, (rank, dev)
+    for r in res:
+        assert r["dev"] <= tol, (r["rank"], r["dev"])
 
 
 def test_process_grid_topology():

@@ -2,15 +2,14 @@
 wil_mat / wil_matpc / clover_mat / clover_matpc (the reference's --test Mat / MatPC / MatPCDagMatPC cases,
 tests/dslash_test_utils.h:363-786) and a host-verified true residual as invert_test does
 (tests/invert_test_gtest.hpp:107-128)."""
-import numpy as np
 import pytest
 
 import oracle
 from common import CudaMem, Problem, assert_close
 from quda_b200 import dirac as DR
+from solvers import KAPPA, MU, X8, busy_default_stream, solve
 
 pytestmark = pytest.mark.gpu
-KAPPA = 0.12195
 
 
 @pytest.mark.parametrize("prec", [8, 4])
@@ -57,53 +56,17 @@ def test_clover_mat_and_matpc(prec, dynamic):
             assert_close(ref, P.to_host(out), prec, 12, f"clover Mpc type={matpc} dag={dagger}")
 
 
-def _solve_full_system(P, kind_pc, X, tol, mixed, matpc=DR.MATPC_EVEN_EVEN, stream=None):
-    """invertQuda-style: prepare -> CG on MpcdagMpc -> reconstruct, then verify M x = b on the host."""
-    import torch
-    kw = dict(clover=P.A, clover_inv=P.Ainv) if "clover" in kind_pc else {}
-    pc = DR.Dirac(kind_pc, P.U, KAPPA, matpc_type=matpc, stream=stream, **kw)
-    b = P.spinor(seed=77, nparity=2)
-    bdev, xdev = P.to_dev(b, 2), P.empty(2)
-    src_p, sol_p = pc.prepare(xdev, bdev)
-    Vh = P.Vh
-    pb = xdev.parity_bytes
-    from quda_b200 import dslash as D
-    src = D.ColorSpinorField(xdev.buf[src_p * pb:(src_p + 1) * pb], X, P.prec)
-    sol = D.ColorSpinorField(xdev.buf[sol_p * pb:(sol_p + 1) * pb], X, P.prec)
-    # normal equations: MdagM sol = Mdag src
-    rhs = P.empty()
-    pc.Mdag(rhs, src)
-    sol.buf.zero_()
-    sloppy = None
-    if mixed:
-        Ps = Problem(X, 4, 12, CudaMem, clover=P.clover is not None, compressed=True, dynamic=True)
-        kws = dict(clover=Ps.A, clover_inv=Ps.Ainv) if "clover" in kind_pc else {}
-        sloppy = DR.Dirac(kind_pc, Ps.U, KAPPA, matpc_type=matpc, stream=stream, **kws)
-        sloppy._keep = Ps
-    res = DR.invert_cg(pc, sloppy, sol, rhs, tol=tol, maxiter=2000)
-    pc.reconstruct(xdev, bdev)
-    x = P.to_host(xdev)
-    if "clover" in kind_pc:
-        Mx = oracle.clover_mat(P.gauge, P.clover, x.astype(b.dtype), X, KAPPA, 0)
-    else:
-        Mx = oracle.wil_mat(P.gauge, x.astype(b.dtype), X, KAPPA, 0)
-    true_res = np.linalg.norm(Mx.astype(np.float64).ravel() - b.astype(np.float64).ravel()) / np.linalg.norm(b.ravel())
-    return res, true_res
-
-
 def test_cg_wilson_double():
-    X = (8, 8, 8, 8)
-    P = Problem(X, 8, 18, CudaMem)
-    res, true_res = _solve_full_system(P, "wilsonpc", X, 1e-10, mixed=False)
+    P = Problem(X8, 8, 18, CudaMem)
+    res, true_res, _, _ = solve(P, "wilsonpc", "cg")
     assert res.iter < 2000 and res.true_res < 5e-10
     assert true_res < 1e-8, true_res  # host-verified residual of the FULL system (normal-equation solve squares the condition)
 
 
 def test_cg_clover_mixed_precision():
     """config 5 in miniature: clover, CG on MdagM, double precise / single sloppy with reliable updates"""
-    X = (8, 8, 8, 8)
-    P = Problem(X, 8, 18, CudaMem, clover=True, compressed=True, dynamic=True)
-    res, true_res = _solve_full_system(P, "cloverpc", X, 1e-10, mixed=True)
+    P = Problem(X8, 8, 18, CudaMem, clover=True, compressed=True, dynamic=True)
+    res, true_res, _, _ = solve(P, "cloverpc", "cg", mixed=True)
     assert res.reliable_updates >= 1
     assert res.true_res < 5e-10, res.true_res
     assert true_res < 1e-8, true_res
@@ -137,9 +100,6 @@ def test_partitioned_operators_through_cpp_layer():
     assert not ex.timed_out()
 
 
-MU = 0.1
-
-
 @pytest.mark.parametrize("prec", [8, 4])
 def test_twisted_mass_mat_and_matpc(prec):
     """DiracTwistedMass / DiracTwistedMassPC (lib/dirac_twisted_mass.cpp) against tm_mat / tm_matpc"""
@@ -164,24 +124,8 @@ def test_twisted_mass_mat_and_matpc(prec):
 @pytest.mark.parametrize("matpc", [DR.MATPC_EVEN_EVEN, DR.MATPC_ODD_ODD_ASYMMETRIC])
 def test_cg_twisted_mass_full_system(matpc):
     """prepare -> CG on MpcdagMpc -> reconstruct for the twisted-mass operator, verified with the oracle's tm_mat"""
-    from quda_b200 import dslash as D
-    X = (8, 8, 8, 8)
-    P = Problem(X, 8, 18, CudaMem)
-    pc = DR.Dirac("twistedmasspc", P.U, KAPPA, matpc_type=matpc, mu=MU)
-    b = P.spinor(seed=77, nparity=2)
-    bdev, xdev = P.to_dev(b, 2), P.empty(2)
-    src_p, sol_p = pc.prepare(xdev, bdev)
-    pb = xdev.parity_bytes
-    src = D.ColorSpinorField(xdev.buf[src_p * pb:(src_p + 1) * pb], X, 8)
-    sol = D.ColorSpinorField(xdev.buf[sol_p * pb:(sol_p + 1) * pb], X, 8)
-    rhs = P.empty()
-    pc.Mdag(rhs, src)
-    sol.buf.zero_()
-    res = DR.invert_cg(pc, None, sol, rhs, tol=1e-10, maxiter=2000)
-    pc.reconstruct(xdev, bdev)
-    x = P.to_host(xdev)
-    Mx = oracle.tm_mat(P.gauge, x, X, KAPPA, MU, 0)
-    true_res = np.linalg.norm(Mx.ravel() - b.ravel()) / np.linalg.norm(b.ravel())
+    P = Problem(X8, 8, 18, CudaMem)
+    res, true_res, _, _ = solve(P, "twistedmasspc", "cg", matpc)
     assert res.iter < 2000 and true_res < 1e-8, (res.iter, true_res)
 
 
@@ -191,17 +135,9 @@ def test_cg_on_a_non_blocking_stream(mixed):
     cudaStreamNonBlocking stream (any torch side stream is one -- it does NOT synchronise with the legacy default stream)
     while the default stream is kept busy with unrelated work, and solve.  With blas kernels on the default stream (the
     round-1 bug) axpyNorm / reDotProduct would race against MdagM and the solve would diverge or return garbage."""
-    import torch
-    X = (8, 8, 8, 8)
-    P = Problem(X, 8, 18, CudaMem, clover=True, compressed=True, dynamic=True)
-    side = torch.cuda.Stream()
-    junk = torch.empty(64 << 20, dtype=torch.float32, device="cuda")
-    torch.cuda.synchronize()
-    for _ in range(20):
-        junk.add_(1.0)  # keeps the default stream busy during the solve
-    with torch.cuda.stream(side):
-        res, true_res = _solve_full_system(P, "cloverpc", X, 1e-10, mixed=mixed, stream=side.cuda_stream)
-        side.synchronize()
+    P = Problem(X8, 8, 18, CudaMem, clover=True, compressed=True, dynamic=True)
+    with busy_default_stream() as side:
+        res, true_res, _, _ = solve(P, "cloverpc", "cg", mixed=mixed, stream=side.cuda_stream)
     assert res.iter < 2000 and res.true_res < 5e-10, (res.iter, res.true_res)
     assert true_res < 1e-8, true_res
     # the host followed the GPU one iteration behind: about one stream synchronisation per iteration, none of them on
@@ -212,8 +148,7 @@ def test_cg_on_a_non_blocking_stream(mixed):
 def test_reductions_are_bit_reproducible():
     """two-stage reductions summed in a fixed order: the same solve twice gives bit-identical iteration counts and
     residuals (the reference needs QUDA_DETERMINISTIC_REDUCE for this, include/communicator_quda.h:570)"""
-    X = (8, 8, 8, 8)
-    P = Problem(X, 8, 18, CudaMem)
-    a = _solve_full_system(P, "wilsonpc", X, 1e-10, mixed=False)
-    b = _solve_full_system(P, "wilsonpc", X, 1e-10, mixed=False)
+    P = Problem(X8, 8, 18, CudaMem)
+    a = solve(P, "wilsonpc", "cg")
+    b = solve(P, "wilsonpc", "cg")
     assert a[0].iter == b[0].iter and a[0].true_res == b[0].true_res and a[1] == b[1]

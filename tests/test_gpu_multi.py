@@ -3,35 +3,18 @@ NVLink (CUDA-IPC peer mapping + arrival flags) -- and the NCCL send/recv fallbac
 Skipped on single-GPU boxes; run explicitly with `gpurun --gpus 2 -- python -m pytest tests/test_gpu_multi.py -m gpu`."""
 import pytest
 import torch
-import torch.multiprocessing as mp
 
-from dist_worker import worker
-from test_dist_gloo import _free_port
+from dist_worker import run_ranks, solver_worker, worker
 
 pytestmark = [pytest.mark.gpu, pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs >= 2 GPUs")]
 
 
 def _run(world, grid_dims, Xl, prec, recon, mode, n_src=1):
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=worker, args=(r, world, port, grid_dims, Xl, prec, recon, q, mode, 6, n_src)) for r in range(world)]
-    for p in procs:
-        p.start()
-    try:
-        res = [q.get(timeout=600) for _ in procs]
-        for p in procs:
-            p.join(timeout=120)
-            assert p.exitcode == 0
-    finally:  # never leave a rank behind on the GPUs (a hung rank would starve every later test)
-        for p in procs:
-            if p.is_alive():
-                p.terminate()
-                p.join(timeout=30)
+    res = run_ranks(worker, world, (grid_dims, Xl, prec, recon, mode, 6, n_src), timeout=600)
     tol = {8: 1e-11, 4: 1e-4, 2: 1e-2}[prec]
-    for rank, dev, timed_out in res:
-        assert not timed_out, f"rank {rank}: exterior kernel timed out waiting for its neighbour"
-        assert dev <= tol, (rank, dev)
+    for r in res:
+        assert not r["timed_out"], f"rank {r['rank']}: exterior kernel timed out waiting for its neighbour"
+        assert r["dev"] <= tol, (r["rank"], r["dev"])
 
 
 @pytest.mark.parametrize("mode", ["p2p-fused", "p2p", "nccl"])
@@ -72,20 +55,10 @@ def test_eight_gpus_three_partitioned_dims():
 def test_two_gpu_cg_host_verified(kind, mixed):
     """config 5 in miniature: CG to 1e-10 on a lattice split over 2 GPUs (clover: double/single mixed precision with
     reliable updates); the gathered solution must satisfy M x = b on the GLOBAL lattice according to the CPU oracle."""
-    from dist_worker import cg_worker
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=cg_worker, args=(r, 2, port, (1, 1, 1, 2), (8, 8, 8, 8), q, mixed, kind)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = [q.get(timeout=900) for _ in procs]
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
-    for rank, iters, rel_updates, solver_res, true_res, timed_out in res:
-        assert not timed_out
-        assert iters < 3000 and solver_res < 5e-10, (iters, solver_res)
-        assert true_res < 1e-8, true_res
+    res = run_ranks(solver_worker, 2, ((1, 1, 1, 2), (8, 8, 8, 8), "cg", kind, mixed), timeout=900)
+    for r in res:
+        assert not r["timed_out"]
+        assert r["iter"] < 3000 and r["true_res"] < 5e-10, (r["iter"], r["true_res"])
+        assert r["host_true_res"] < 1e-8, r["host_true_res"]
         if mixed:
-            assert rel_updates >= 1
+            assert r["reliable_updates"] >= 1

@@ -8,82 +8,22 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import oracle
 from common import CudaMem, Problem
 from quda_b200 import dirac as DR
 from quda_b200 import lib as L
-from test_gpu_bicgstab import KAPPA, MU, X8, _ops
+from solvers import (CASE_IDS, CASES, KAPPA, OFFSETS, X8, busy_default_stream, check_shifts, operators, self_exchanges,
+                     set_host_allreduce, shift_residual, solve_multishift)
 
 pytestmark = pytest.mark.gpu
-OFFSETS = [0.0, 1e-3, 1e-2, 0.1, 1.0, 10.0]
-
-
-def _normal_op(P, kind, matpc, x, kappa=KAPPA):
-    """M^dag M x with the oracle in fp64 (the preconditioned operator for the *pc types, the full one otherwise)"""
-    x = x.astype(np.float64)
-    if kind == "wilsonpc":
-        m = lambda v, d: oracle.wil_matpc(P.gauge, v, P.X, kappa, matpc, d)  # noqa: E731
-    elif kind == "cloverpc":
-        m = lambda v, d: oracle.clover_matpc(P.gauge, P.clover, P.clover_inv, v, P.X, kappa, matpc, d)  # noqa: E731
-    elif kind == "twistedmasspc":
-        m = lambda v, d: oracle.tm_matpc(P.gauge, v, P.X, kappa, MU, matpc, d)  # noqa: E731
-    elif kind == "wilson":
-        m = lambda v, d: oracle.wil_mat(P.gauge, v, P.X, kappa, d)  # noqa: E731
-    else:
-        m = lambda v, d: oracle.clover_mat(P.gauge, P.clover, v, P.X, kappa, d)  # noqa: E731
-    return m(m(x, 0), 1)
-
-
-def _shift_residual(P, kind, matpc, x, b, sigma, kappa=KAPPA):
-    """|(M^dag M + sigma) x - b| / |b| on the host in fp64"""
-    r = _normal_op(P, kind, matpc, x, kappa) + sigma * x.astype(np.float64) - b.astype(np.float64)
-    return float(np.linalg.norm(r.ravel()) / np.linalg.norm(b.ravel()))
-
-
-def _ms(P, kind, offsets, matpc=DR.MATPC_EVEN_EVEN, mixed=False, kappa=KAPPA, tol=1e-10, tol_offset=None, stream=None,
-        comm=None, seed=77, b=None, xs=None, maxiter=2000, ops=None):
-    """multi-shift solve; returns (result, [x_j on the host], b on the host as the device holds it)"""
-    precise, sloppy = ops or _ops(P, kind, matpc, kappa, mixed, stream, comm)
-    npar = 1 if kind.endswith("pc") else 2
-    if b is None:
-        b = P.spinor(seed=seed, nparity=npar)
-    bdev = P.to_dev(b, npar)
-    if xs is None:
-        xs = [P.empty(npar) for _ in offsets]
-    res = DR.invert_multishift_cg(precise, sloppy, xs, bdev, offsets, tol=tol, tol_offset=tol_offset, maxiter=maxiter)
-    return res, [P.to_host(x) for x in xs], b
-
-
-def _check_shifts(P, kind, matpc, res, xs, b, offsets, tols, kappa=KAPPA, bound=1e-8):
-    for j, (sigma, x) in enumerate(zip(offsets, xs)):
-        assert np.isfinite(x).all(), j
-        rr = _shift_residual(P, kind, matpc, x, b, sigma, kappa)
-        assert rr < bound, (j, sigma, rr)
-        assert res.true_res_offset[j] <= tols[j], (j, res.true_res_offset[j], tols[j])
-        assert np.isfinite(res.iter_res_offset[j]), j
-        assert 0 <= res.iter_offset[j] <= res.iter, (j, res.iter_offset[j], res.iter)
-
-
-CASES = [
-    ("wilsonpc", dict(), DR.MATPC_EVEN_EVEN),
-    ("wilsonpc", dict(), DR.MATPC_ODD_ODD_ASYMMETRIC),
-    ("cloverpc", dict(clover=True, compressed=True, dynamic=True), DR.MATPC_EVEN_EVEN),
-    ("cloverpc", dict(clover=True, compressed=False, dynamic=False), DR.MATPC_EVEN_EVEN),
-    ("cloverpc", dict(clover=True, compressed=False, dynamic=False), DR.MATPC_ODD_ODD_ASYMMETRIC),
-    ("cloverpc", dict(clover=True, compressed=True, dynamic=True), DR.MATPC_EVEN_EVEN_ASYMMETRIC),
-    ("twistedmasspc", dict(), DR.MATPC_EVEN_EVEN),
-    ("twistedmasspc", dict(), DR.MATPC_ODD_ODD_ASYMMETRIC),
-]
 
 
 @pytest.mark.parametrize("mixed", [False, True], ids=["fp64", "fp64-fp32"])
-@pytest.mark.parametrize("kind,pkw,matpc", CASES, ids=[f"{k}-{'dyn' if p.get('dynamic') else ('static' if p else 'plain')}-matpc{m}"
-                                                      for k, p, m in CASES])
+@pytest.mark.parametrize("kind,pkw,matpc", CASES, ids=CASE_IDS)
 def test_multishift_preconditioned_system(kind, pkw, matpc, mixed):
     P = Problem(X8, 8, 18, CudaMem, **pkw)
-    res, xs, b = _ms(P, kind, OFFSETS, matpc, mixed)
+    res, xs, b = solve_multishift(P, kind, OFFSETS, matpc, mixed)
     assert 0 < res.iter < 2000, res.iter
-    _check_shifts(P, kind, matpc, res, xs, b, OFFSETS, [1e-10] * len(OFFSETS))
+    check_shifts(P, kind, matpc, res, xs, b, OFFSETS, [1e-10] * len(OFFSETS))
     if mixed:
         assert res.reliable_updates >= 1, res.reliable_updates
     else:
@@ -94,20 +34,20 @@ def test_multishift_preconditioned_system(kind, pkw, matpc, mixed):
 @pytest.mark.parametrize("kind", ["wilson", "clover"])
 def test_multishift_full_system(kind):
     P = Problem(X8, 8, 18, CudaMem, clover=kind == "clover", compressed=True, dynamic=True)
-    res, xs, b = _ms(P, kind, OFFSETS)
-    _check_shifts(P, kind, None, res, xs, b, OFFSETS, [1e-10] * len(OFFSETS))
+    res, xs, b = solve_multishift(P, kind, OFFSETS)
+    check_shifts(P, kind, None, res, xs, b, OFFSETS, [1e-10] * len(OFFSETS))
 
 
 @pytest.mark.parametrize("mixed", [False, True], ids=["fp64", "fp64-fp32"])
 def test_multishift_is_cheaper_than_sequential_solves(mixed):
     """one recursion for all shifts (plus its refinements) against one single-shift solve per shift"""
     P = Problem(X8, 8, 18, CudaMem, clover=True, compressed=True, dynamic=True)
-    ops = _ops(P, "cloverpc", DR.MATPC_EVEN_EVEN, mixed=mixed)
-    ms, xs, b = _ms(P, "cloverpc", OFFSETS, ops=ops)
+    ops = operators(P, "cloverpc", DR.MATPC_EVEN_EVEN, mixed=mixed)
+    ms, xs, b = solve_multishift(P, "cloverpc", OFFSETS, ops=ops)
     seq = 0
     for j, sigma in enumerate(OFFSETS):
-        one, (x1,), _ = _ms(P, "cloverpc", [sigma], b=b, ops=ops)
-        assert _shift_residual(P, "cloverpc", DR.MATPC_EVEN_EVEN, x1, b, sigma) < 1e-8
+        one, (x1,), _ = solve_multishift(P, "cloverpc", [sigma], b=b, ops=ops)
+        assert shift_residual(P, "cloverpc", DR.MATPC_EVEN_EVEN, x1, b, sigma) < 1e-8
         seq += one.iter + one.refine_iter[0]
     total = ms.iter + sum(ms.refine_iter[:len(OFFSETS)])
     print(f"multi-shift {ms.iter} + refinement {list(ms.refine_iter[:len(OFFSETS)])} vs sequential {seq}")
@@ -117,37 +57,37 @@ def test_multishift_is_cheaper_than_sequential_solves(mixed):
 
 def test_shift_zero_agrees_with_cg():
     P = Problem(X8, 8, 18, CudaMem, clover=True, compressed=True, dynamic=True)
-    precise, _ = _ops(P, "cloverpc", DR.MATPC_EVEN_EVEN)
-    ms, xs, b = _ms(P, "cloverpc", [0.0, 0.01, 0.1], ops=(precise, None))
+    precise, _ = operators(P, "cloverpc", DR.MATPC_EVEN_EVEN)
+    ms, xs, b = solve_multishift(P, "cloverpc", [0.0, 0.01, 0.1], ops=(precise, None))
     x = P.empty()
     cg = DR.invert_cg(precise, None, x, P.to_dev(b), tol=1e-10, maxiter=2000)
     x_cg = P.to_host(x)
     assert abs(ms.iter - cg.iter) <= 1, (ms.iter, cg.iter)
     assert ms.iter_offset[0] == ms.iter
     assert np.linalg.norm(xs[0] - x_cg) / np.linalg.norm(x_cg) < 1e-7
-    assert _shift_residual(P, "cloverpc", DR.MATPC_EVEN_EVEN, xs[0], b, 0.0) < 1e-8
+    assert shift_residual(P, "cloverpc", DR.MATPC_EVEN_EVEN, xs[0], b, 0.0) < 1e-8
 
 
 def test_per_shift_tolerances_retire_shifts_early():
     P = Problem(X8, 8, 18, CudaMem, clover=True, compressed=True, dynamic=True)
     offsets = [0.0, 0.01, 0.1, 1.0]
-    tight, _, _ = _ms(P, "cloverpc", offsets)
+    tight, _, _ = solve_multishift(P, "cloverpc", offsets)
     loose_tols = [1e-10, 1e-10, 1e-4, 1e-4]
-    loose, xs, b = _ms(P, "cloverpc", offsets, tol_offset=loose_tols)
-    _check_shifts(P, "cloverpc", DR.MATPC_EVEN_EVEN, loose, xs, b, offsets, loose_tols, bound=1.0)
+    loose, xs, b = solve_multishift(P, "cloverpc", offsets, tol_offset=loose_tols)
+    check_shifts(P, "cloverpc", DR.MATPC_EVEN_EVEN, loose, xs, b, offsets, loose_tols, bound=1.0)
     for j in (0, 1):
-        assert _shift_residual(P, "cloverpc", DR.MATPC_EVEN_EVEN, xs[j], b, offsets[j]) < 1e-8
+        assert shift_residual(P, "cloverpc", DR.MATPC_EVEN_EVEN, xs[j], b, offsets[j]) < 1e-8
     for j in (2, 3):
         assert loose.iter_offset[j] < tight.iter_offset[j], (j, list(loose.iter_offset[:4]), list(tight.iter_offset[:4]))
         assert loose.iter_offset[j] < loose.iter_offset[0]
-        assert _shift_residual(P, "cloverpc", DR.MATPC_EVEN_EVEN, xs[j], b, offsets[j]) < 2e-4
+        assert shift_residual(P, "cloverpc", DR.MATPC_EVEN_EVEN, xs[j], b, offsets[j]) < 2e-4
     assert loose.iter_offset[3] <= loose.iter_offset[2] <= loose.iter_offset[1] <= loose.iter_offset[0] == loose.iter
 
 
 def test_zero_source_gives_zero_solutions():
     P = Problem(X8, 8, 18, CudaMem)
     xs = [P.to_dev(P.spinor(seed=5 + j)) for j in range(3)]  # non-zero on entry
-    res, out, _ = _ms(P, "wilsonpc", [0.0, 0.1, 1.0], b=np.zeros_like(P.spinor()), xs=xs)
+    res, out, _ = solve_multishift(P, "wilsonpc", [0.0, 0.1, 1.0], b=np.zeros_like(P.spinor()), xs=xs)
     assert res.iter == 0
     for x in out:
         assert not x.any()
@@ -158,7 +98,7 @@ def test_kappa_zero_one_iteration():
     alpha_j = 1 / (1 + sigma_j) from the zeta recursion"""
     P = Problem(X8, 8, 18, CudaMem)
     offsets = [0.0, 1e-3, 0.1, 1.0, 10.0]
-    res, xs, b = _ms(P, "wilsonpc", offsets, kappa=0.0)
+    res, xs, b = solve_multishift(P, "wilsonpc", offsets, kappa=0.0)
     assert res.iter == 1, res.iter
     b_dev = P.to_host(P.to_dev(b))  # the native order is a rotated gamma basis: compare with b as the device holds it
     for j, sigma in enumerate(offsets):
@@ -172,24 +112,24 @@ def test_kappa_zero_one_iteration():
 def test_one_and_thirty_two_shifts(n):
     P = Problem(X8, 8, 18, CudaMem, clover=True, compressed=True, dynamic=True)
     offsets = [0.05] if n == 1 else [0.0] + list(np.geomspace(1e-4, 10.0, n - 1))
-    res, xs, b = _ms(P, "cloverpc", offsets, mixed=True)
-    _check_shifts(P, "cloverpc", DR.MATPC_EVEN_EVEN, res, xs, b, offsets, [1e-10] * n)
+    res, xs, b = solve_multishift(P, "cloverpc", offsets, mixed=True)
+    check_shifts(P, "cloverpc", DR.MATPC_EVEN_EVEN, res, xs, b, offsets, [1e-10] * n)
 
 
 def test_duplicate_offsets():
     P = Problem(X8, 8, 18, CudaMem, clover=True, compressed=True, dynamic=True)
     offsets = [0.0, 0.1, 0.1, 1.0, 1.0]
-    res, xs, b = _ms(P, "cloverpc", offsets)
-    _check_shifts(P, "cloverpc", DR.MATPC_EVEN_EVEN, res, xs, b, offsets, [1e-10] * len(offsets))
+    res, xs, b = solve_multishift(P, "cloverpc", offsets)
+    check_shifts(P, "cloverpc", DR.MATPC_EVEN_EVEN, res, xs, b, offsets, [1e-10] * len(offsets))
     assert np.array_equal(xs[1], xs[2]) and np.array_equal(xs[3], xs[4])
 
 
 def test_initial_guess_is_ignored():
     P = Problem(X8, 8, 18, CudaMem, clover=True, compressed=True, dynamic=True)
-    ops = _ops(P, "cloverpc", DR.MATPC_EVEN_EVEN, mixed=True)
-    ref, x_ref, b = _ms(P, "cloverpc", OFFSETS, ops=ops)
+    ops = operators(P, "cloverpc", DR.MATPC_EVEN_EVEN, mixed=True)
+    ref, x_ref, b = solve_multishift(P, "cloverpc", OFFSETS, ops=ops)
     dirty = [P.to_dev(P.spinor(seed=100 + j)) for j in range(len(OFFSETS))]
-    res, xs, _ = _ms(P, "cloverpc", OFFSETS, ops=ops, b=b, xs=dirty)
+    res, xs, _ = solve_multishift(P, "cloverpc", OFFSETS, ops=ops, b=b, xs=dirty)
     assert res.iter == ref.iter
     for a, c in zip(xs, x_ref):
         assert np.array_equal(a, c)
@@ -197,8 +137,8 @@ def test_initial_guess_is_ignored():
 
 def test_multishift_is_bit_reproducible():
     P = Problem(X8, 8, 18, CudaMem, clover=True, compressed=True, dynamic=True)
-    a = _ms(P, "cloverpc", OFFSETS, mixed=True)
-    c = _ms(P, "cloverpc", OFFSETS, mixed=True)
+    a = solve_multishift(P, "cloverpc", OFFSETS, mixed=True)
+    c = solve_multishift(P, "cloverpc", OFFSETS, mixed=True)
     assert a[0].iter == c[0].iter and list(a[0].true_res_offset) == list(c[0].true_res_offset)
     for x, y in zip(a[1], c[1]):
         assert np.array_equal(x, y)
@@ -212,20 +152,14 @@ def _sync_bound(res, n, host_waits=1):
 def test_host_allreduce_matches_the_device_path(mixed):
     """a self-partitioned exchange with an identity callback and no mailbox ranks sends every global sum through the host;
     the host derives the scalars with the same function the finalisers run"""
-    from quda_b200 import comm
     P = Problem(X8, 8, 12, CudaMem, clover=True, compressed=True, dynamic=True)
-    grid = comm.ProcessGrid((1, 1, 1, 1), 0)
-    exs = {p: comm.HaloExchange(grid, P.X, p, mode="self") for p in (8, 4)}
-    css = {p: e.comm_struct() for p, e in exs.items()}
-    identity = L.ALLREDUCE_FN(lambda data, n, user: None)  # one rank: the global sum is the local one
+    exs, css = self_exchanges(P.X)
     n = len(OFFSETS)
     out = {}
     for callback in (False, True):
-        for cs in css.values():
-            assert cs.n_ranks == 0
-            cs.allreduce_sum = C.cast(identity, C.c_void_p) if callback else None
-        res, xs, b = _ms(P, "cloverpc", OFFSETS, mixed=mixed, comm=css)
-        _check_shifts(P, "cloverpc", DR.MATPC_EVEN_EVEN, res, xs, b, OFFSETS, [1e-10] * n)
+        set_host_allreduce(css, callback)
+        res, xs, b = solve_multishift(P, "cloverpc", OFFSETS, mixed=mixed, comm=css)
+        check_shifts(P, "cloverpc", DR.MATPC_EVEN_EVEN, res, xs, b, OFFSETS, [1e-10] * n)
         assert res.host_syncs <= _sync_bound(res, n, 2 if callback else 1), (callback, res.host_syncs, res.iter)
         assert not any(e.timed_out() for e in exs.values())
         out[callback] = (res, xs)
@@ -241,30 +175,20 @@ def test_host_allreduce_matches_the_device_path(mixed):
 @pytest.mark.parametrize("mixed", [False, True], ids=["fp64", "fp64-fp32"])
 def test_multishift_on_a_non_blocking_stream(mixed):
     """every kernel on the operator's stream while the default stream is kept busy; the host follows one iteration behind"""
-    import torch
     P = Problem(X8, 8, 18, CudaMem, clover=True, compressed=True, dynamic=True)
-    side = torch.cuda.Stream()
-    junk = torch.empty(64 << 20, dtype=torch.float32, device="cuda")
-    torch.cuda.synchronize()
-    for _ in range(20):
-        junk.add_(1.0)
-    with torch.cuda.stream(side):
-        res, xs, b = _ms(P, "cloverpc", OFFSETS, mixed=mixed, stream=side.cuda_stream)
-        side.synchronize()
-    _check_shifts(P, "cloverpc", DR.MATPC_EVEN_EVEN, res, xs, b, OFFSETS, [1e-10] * len(OFFSETS))
+    with busy_default_stream() as side:
+        res, xs, b = solve_multishift(P, "cloverpc", OFFSETS, mixed=mixed, stream=side.cuda_stream)
+    check_shifts(P, "cloverpc", DR.MATPC_EVEN_EVEN, res, xs, b, OFFSETS, [1e-10] * len(OFFSETS))
     assert res.host_syncs <= _sync_bound(res, len(OFFSETS)), (res.host_syncs, res.iter, res.reliable_updates)
 
 
 def test_multishift_self_partitioned():
     """one GPU that is its own neighbour in every dimension: every Dslash goes through pack + ghost, one exchange per
     precision"""
-    from quda_b200 import comm
     P = Problem(X8, 8, 12, CudaMem, clover=True, compressed=True, dynamic=True)
-    grid = comm.ProcessGrid((1, 1, 1, 1), 0)
-    exs = {p: comm.HaloExchange(grid, P.X, p, mode="self") for p in (8, 4)}
-    css = {p: e.comm_struct() for p, e in exs.items()}
-    res, xs, b = _ms(P, "cloverpc", OFFSETS, mixed=True, comm=css)
-    _check_shifts(P, "cloverpc", DR.MATPC_EVEN_EVEN, res, xs, b, OFFSETS, [1e-10] * len(OFFSETS))
+    exs, css = self_exchanges(P.X)
+    res, xs, b = solve_multishift(P, "cloverpc", OFFSETS, mixed=True, comm=css)
+    check_shifts(P, "cloverpc", DR.MATPC_EVEN_EVEN, res, xs, b, OFFSETS, [1e-10] * len(OFFSETS))
     assert res.reliable_updates >= 1
     assert not any(e.timed_out() for e in exs.values())
 

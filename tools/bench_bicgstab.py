@@ -12,26 +12,8 @@ reliable updates (BiCGStab: including restarts), time to solution, GFLOP/s with 
 true residual from the unpreconditioned fp64 operator, and the card and its power limit."""
 import argparse
 import json
-import os
-import subprocess
-import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-import bench  # noqa: E402  (field helpers: random SU(3) links, ghost links, device clover)
-
-
-def card():
-    import torch
-    out = {"name": torch.cuda.get_device_name(), "power_limit_w": None}
-    try:
-        q = subprocess.check_output(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i",
-                                     str(torch.cuda.current_device())], timeout=10).decode().strip()
-        out["power_limit_w"] = float(q)
-    except Exception as e:  # noqa: BLE001
-        out["power_limit_w"] = f"unavailable ({e.__class__.__name__})"
-    return out
+from solver_bench import card, max_over_ranks, setup, timed_runs
 
 
 def main():
@@ -43,40 +25,10 @@ def main():
     a = ap.parse_args()
 
     import torch
-    from quda_b200 import comm, dirac as DR, dslash as D, fields as F
-    rank = int(os.environ.get("RANK", "0"))
-    world = int(os.environ.get("WORLD_SIZE", "1"))
-    local_rank = int(os.environ.get("LOCAL_RANK", "0"))
-    assert torch.cuda.is_available(), "bench_bicgstab.py needs a CUDA device (no CPU fallback)"
-    torch.cuda.set_device(local_rank)
-    dist = None
-    if world > 1:
-        import torch.distributed as dist
-        dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
-    dims = comm.ProcessGrid.default_dims(world)
-    grid = comm.ProcessGrid(dims, rank) if world > 1 else None
+    from quda_b200 import dirac as DR, dslash as D, fields as F
+    rank, world, dist, dims, X, ops = setup(a.global_dim, a.kappa)
     Xg = a.global_dim
-    X = [Xg[d] // dims[d] for d in range(4)]
-    assert all(X[d] * dims[d] == Xg[d] and X[d] % 2 == 0 for d in range(4)), f"global lattice {Xg} does not split over {dims}"
-    torch.manual_seed(4321 + rank)
-    u = bench.random_su3_device(X)
-    faces = bench.boundary_links_from_neighbours(u, X, grid)
-    ops, keep = {}, []
     stream = torch.cuda.current_stream().cuda_stream
-    for prec, recon in ((8, 18), (4, 12)):
-        gbuf, gmeta = F.gauge_to_native_torch(u, X, prec, recon, ghost_faces=faces)
-        U = D.GaugeField(gbuf, X, prec, recon, gmeta, anisotropy=1.0, t_boundary=-1,
-                         first_time_slice=grid.first_time_slice() if grid else True,
-                         last_time_slice=grid.last_time_slice() if grid else True)
-        A = bench.device_clover(X, prec)
-        cs = None
-        if world > 1:
-            ex = comm.HaloExchange(grid, X, prec, mode="p2p", dist=dist)
-            cs = ex.comm_struct()
-            keep += [ex, cs]
-        ops[prec] = DR.Dirac("cloverpc", U, a.kappa, clover=A, comm=cs, stream=stream)
-        keep += [U, A]
-    del u
     pc = ops[8]
     pb = F.spinor_bytes(X, 8)
     g = torch.Generator(device="cuda").manual_seed(99 + rank)
@@ -112,30 +64,13 @@ def main():
         return float((nrm[0] / nrm[1]).sqrt())
 
     solvers = ("cg", "bicgstab")
-    for s in solvers:
-        solve(s)  # warm-up: first-use allocations, clocks
     runs = {s: [] for s in solvers}
-    for _ in range(a.reps):
-        for s in solvers:
-            if world > 1:
-                dist.barrier()
-            torch.cuda.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            res = solve(s)
-            e1.record()
-            torch.cuda.synchronize()
-            secs = e0.elapsed_time(e1) * 1e-3
-            runs[s].append((secs, res, true_residual()))
+    for s, secs, res in timed_runs(solvers, solve, a.reps, dist):
+        runs[s].append((secs, res, true_residual()))
     info = card()
     for s in solvers:
         secs, res, tr = min(runs[s], key=lambda r: r[0])
-        if world > 1:
-            t = torch.tensor([secs, res.secs], device="cuda", dtype=torch.float64)
-            dist.all_reduce(t, op=dist.ReduceOp.MAX)
-            secs, solver_secs = float(t[0]), float(t[1])
-        else:
-            solver_secs = res.secs
+        secs, solver_secs = max_over_ranks(dist, secs, res.secs)
         # residual recomputations in the precise operator: the initial and final one and one per reliable update, each
         # M^dag M (2 M) for CG and M for BiCGStab; BiCGStab also applies M twice in the iteration queued behind the one
         # that converged (its BLAS kernels return at once)

@@ -19,15 +19,9 @@ achieved bandwidth uses the (1 + 4 n) S byte model (S = one single-parity fp32 s
 sheet's 3.35 TB/s."""
 import argparse
 import json
-import os
 import statistics
-import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-import bench  # noqa: E402  (field helpers: random SU(3) links, ghost links, device clover)
-from bench_bicgstab import card  # noqa: E402
+from solver_bench import card, max_over_ranks, setup, timed_runs
 
 # 12 poles over 1e-4 .. 10, as a rational approximation for RHMC has them
 OFFSETS = [1e-4 * (1e5 ** (j / 11)) for j in range(12)]
@@ -54,40 +48,9 @@ def main():
     a = ap.parse_args()
 
     import torch
-    from quda_b200 import comm, dirac as DR, dslash as D, fields as F
-    rank = int(os.environ.get("RANK", "0"))
-    world = int(os.environ.get("WORLD_SIZE", "1"))
-    local_rank = int(os.environ.get("LOCAL_RANK", "0"))
-    assert torch.cuda.is_available(), "bench_multishift.py needs a CUDA device (no CPU fallback)"
-    torch.cuda.set_device(local_rank)
-    dist = None
-    if world > 1:
-        import torch.distributed as dist
-        dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
-    dims = comm.ProcessGrid.default_dims(world)
-    grid = comm.ProcessGrid(dims, rank) if world > 1 else None
+    from quda_b200 import dirac as DR, dslash as D, fields as F
+    rank, world, dist, dims, X, ops = setup(a.global_dim, a.kappa)
     Xg = a.global_dim
-    X = [Xg[d] // dims[d] for d in range(4)]
-    assert all(X[d] * dims[d] == Xg[d] and X[d] % 2 == 0 for d in range(4)), f"global lattice {Xg} does not split over {dims}"
-    torch.manual_seed(4321 + rank)
-    u = bench.random_su3_device(X)
-    faces = bench.boundary_links_from_neighbours(u, X, grid)
-    ops, keep = {}, []
-    stream = torch.cuda.current_stream().cuda_stream
-    for prec, recon in ((8, 18), (4, 12)):
-        gbuf, gmeta = F.gauge_to_native_torch(u, X, prec, recon, ghost_faces=faces)
-        U = D.GaugeField(gbuf, X, prec, recon, gmeta, anisotropy=1.0, t_boundary=-1,
-                         first_time_slice=grid.first_time_slice() if grid else True,
-                         last_time_slice=grid.last_time_slice() if grid else True)
-        A = bench.device_clover(X, prec)
-        cs = None
-        if world > 1:
-            ex = comm.HaloExchange(grid, X, prec, mode="p2p", dist=dist)
-            cs = ex.comm_struct()
-            keep += [ex, cs]
-        ops[prec] = DR.Dirac("cloverpc", U, a.kappa, clover=A, comm=cs, stream=stream)
-        keep += [U, A]
-    del u
     pc = ops[8]
     sloppy = ops[4] if a.sloppy == "single" else None
     pb = F.spinor_bytes(X, 8)
@@ -105,27 +68,13 @@ def main():
         return [DR.invert_multishift_cg(pc, sloppy, [x], b, [s], tol=a.tol, maxiter=20000) for s, x in zip(OFFSETS, xs)]
 
     modes = ("multishift", "sequential")
-    for m in modes:
-        solve(m)  # warm-up: first-use allocations, clocks
     runs = {m: [] for m in modes}
-    for _ in range(a.reps):
-        for m in modes:
-            if world > 1:
-                dist.barrier()
-            torch.cuda.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            res = solve(m)
-            e1.record()
-            torch.cuda.synchronize()
-            runs[m].append((e0.elapsed_time(e1) * 1e-3, res))
+    for m, secs, res in timed_runs(modes, solve, a.reps, dist):
+        runs[m].append((secs, res))
     info = card()
     for m in modes:
         secs, res = min(runs[m], key=lambda r: r[0])
-        if world > 1:
-            t = torch.tensor([secs], device="cuda", dtype=torch.float64)
-            dist.all_reduce(t, op=dist.ReduceOp.MAX)
-            secs = float(t[0])
+        secs, = max_over_ranks(dist, secs)
         if m == "multishift":
             r, n = res[0], len(OFFSETS)
             iters, refine = r.iter, list(r.refine_iter[:n])
