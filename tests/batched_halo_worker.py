@@ -1,7 +1,7 @@
 """GPU worker of tests/test_gpu_batched_halo.py (run as a subprocess so that a device fault cannot take the rest of the GPU
 tier with it): the batched multi-RHS halo (b200_pack_ghost_multi) on one GPU that is its own neighbour.
-  1. PackGhostMulti + per-source Dslash on plain ghost buffers (arrival by stream order) -- tests/ops.py, the same case
-     list the host twin runs in the CPU tier;
+  1. PackGhostMulti + per-source Dslash on plain ghost buffers (arrival by stream order) -- ops.check_partitioned_multi,
+     the case body the host twin runs in the CPU tier (tests/test_twin_ops.py::test_batched_halo_*);
   2. HaloExchange(mode="self", n_src=...): the arrival-counter protocol (one signal per face for the whole batch), batched
      and single exchanges interleaved on the same double-buffered slabs.
 Prints one line per case and "ALL OK" at the end."""

@@ -86,6 +86,7 @@ class Problem:
         self.U = D.GaugeField(mem.put(gbuf), X, prec, recon, gmeta, anisotropy=anisotropy,
                               t_boundary=-1 if antiperiodic_t else 1)
         self.clover = self.clover_inv = self.A = self.Ainv = None
+        self.dynamic = dynamic
         if clover:
             self.clover = oracle.random_clover(X, hp, seed=seed + 1)
             self.clover_inv = oracle.clover_invert(self.clover)

@@ -142,6 +142,7 @@ def worker(rank, world, port, q, grid_dims, Xl, prec, recon, mode="host", reps=3
         mode = "p2p"
     dist = _join(rank, world, port, "gloo" if mode == "host" else "nccl")
     import oracle
+    import ops
     from common import CudaMem, HostMem, twin_backend
     from quda_b200 import comm
     be = twin_backend() if mode == "host" else None
@@ -153,7 +154,7 @@ def worker(rank, world, port, q, grid_dims, Xl, prec, recon, mode="host", reps=3
     parity, dagger, kappa = 1, 0, 0.12195
     s = oracle.random_spinor(Xg, hp, seed=5)
     xs = oracle.random_spinor(Xg, hp, seed=6)
-    ref = xs.astype(np.float64) - kappa * oracle.wil_dslash(gauge, s, Xg, parity, dagger).astype(np.float64)
+    ref = ops.xpay(xs, -kappa, oracle.wil_dslash(gauge, s, Xg, parity, dagger))
     U = blk.gauge_field(gauge, prec, recon)
     din, dx, out = blk.spinor_field(s, prec, 1 - parity), blk.spinor_field(xs, prec, parity), blk.empty(prec)
     if n_src > 1:
@@ -169,7 +170,7 @@ def worker(rank, world, port, q, grid_dims, Xl, prec, recon, mode="host", reps=3
         dev = 0.0
         for i in range(n_src + 1):
             v, o = (srcs[i], outs[i]) if i < n_src else (s, out)
-            r = xs.astype(np.float64) - kappa * oracle.wil_dslash(gauge, v, Xg, parity, dagger).astype(np.float64)
+            r = ops.xpay(xs, -kappa, oracle.wil_dslash(gauge, v, Xg, parity, dagger))
             dev = max(dev, oracle.compare_spinor(comm.local_slice(r, Xg, Xl, grid.coords, ("spinor1", parity)), blk.to_host(o))[1])
     else:
         ex = comm.HaloExchange(grid, Xl, prec, mode=mode, backend=be, dist=dist)

@@ -24,20 +24,17 @@ class Fields:
         self.U = D.GaugeField(mem.put(gbuf), X, prec, recon, gmeta, anisotropy=anisotropy, t_boundary=tb)
         self.G = PR.decode_gauge(gbuf, X, prec, recon, gmeta, anisotropy, tb)
         self.dynamic = dynamic
+        self.image = {}  # device clover field -> the decoded field the kernel reads
         if clover is not None:
             host = oracle.random_clover(X, 8, seed=seed + 1) if clover == "near" else PR.hpd_clover(X, seed + 1, clover)
             self.clover = host
             cbuf, cmeta = F.clover_to_native(host, X, prec, compressed=compressed)
-            self.Adev = D.CloverField(mem.put(cbuf), X, prec, cmeta, dynamic=True)
-            self.A = PR.decode_clover(cbuf, X, prec, cmeta)
+            self.A = D.CloverField(mem.put(cbuf), X, prec, cmeta, dynamic=True)
+            self.image[self.A] = PR.decode_clover(cbuf, X, prec, cmeta)
             if not dynamic:
                 ibuf, imeta = F.clover_to_native(oracle.clover_invert(np.ascontiguousarray(host)), X, prec, compressed=False)
-                self.Ainv_dev = D.CloverField(mem.put(ibuf), X, prec, imeta, dynamic=False)
-                self.Ainv = PR.decode_clover(ibuf, X, prec, imeta)
-
-    def inv_field(self):
-        """(device field, decoded field) that A^-1 is taken from"""
-        return (self.Adev, self.A) if self.dynamic else (self.Ainv_dev, self.Ainv)
+                self.Ainv = D.CloverField(mem.put(ibuf), X, prec, imeta, dynamic=False)
+                self.image[self.Ainv] = PR.decode_clover(ibuf, X, prec, imeta)
 
     def spinor(self, host):
         """oracle-order host spinor (one parity) -> (native field, decoded native-basis value the kernel reads)"""
@@ -63,17 +60,9 @@ def spinor_kind(X, kind, seed, prec):
     return PR.gaussian_spinor(X, seed, points=sorted({0, Vh // 3, Vh - 1, (7 * Vh) // 11}))
 
 
-def apply_op(Fs, op, be, parity, dagger, din, xd=None, a=0.0, halo=None, mu=0.1, kappa=0.12195, **kw):
+def apply_op(Fs, op, be, parity, dagger, din, xd=None, a=0.0, **kw):
     out = Fs.empty()
-    if op == "wilson":
-        D.ApplyWilson(out, din, Fs.U, a, xd, parity, dagger, halo=halo, backend=be, **kw)
-    elif op == "clover":
-        D.ApplyWilsonClover(out, din, Fs.U, Fs.Adev, a, xd, parity, dagger, halo=halo, backend=be, **kw)
-    elif op == "clover_pc":
-        D.ApplyWilsonCloverPreconditioned(out, din, Fs.U, Fs.inv_field()[0], a, xd, parity, dagger, halo=halo, backend=be,
-                                          **kw)
-    elif op == "tm":
-        D.ApplyTwistedMass(out, din, Fs.U, a, 2 * kappa * mu, xd, parity, dagger, halo=halo, backend=be, **kw)
+    ops.apply(Fs, op, out, din, a, xd, parity, dagger, backend=be, **kw)
     return out
 
 
@@ -82,9 +71,9 @@ def reference(Fs, op, parity, dagger, psi, x=None, a=0.0, ghosts=None, mu=0.1, k
     if op == "wilson":
         return PR.wilson(Fs.G, psi, Fs.X, parity, dagger, p, a, x, ghosts)
     if op == "clover":
-        return PR.wilson_clover(Fs.G, Fs.A, psi, Fs.X, parity, dagger, p, a, x, ghosts)
+        return PR.wilson_clover(Fs.G, Fs.image[Fs.A], psi, Fs.X, parity, dagger, p, a, x, ghosts)
     if op == "clover_pc":
-        return PR.clover_pc(Fs.G, Fs.inv_field()[1], psi, Fs.X, parity, dagger, p, Fs.dynamic, a, x, ghosts)
+        return PR.clover_pc(Fs.G, Fs.image[ops.clover_inverse(Fs)], psi, Fs.X, parity, dagger, p, Fs.dynamic, a, x, ghosts)
     if op == "tm":
         return PR.twisted_mass(Fs.G, psi, Fs.X, parity, dagger, p, a, 2 * kappa * mu, x)
     raise ValueError(op)
@@ -96,10 +85,12 @@ def check_op(Fs, op, be, parity=0, dagger=0, kind="gauss", xpay=False, seed=5, w
     din, psi = Fs.spinor(psi_h)
     xd = x = None
     a = 0.0
-    if xpay or op in ("clover", "tm"):
+    if ops.takes_x(op, xpay):
         xd, x = Fs.spinor(spinor_kind(Fs.X, kind, seed + 1, Fs.prec))
         a = -0.12195
-    out = apply_op(Fs, op, be, parity, dagger, din, xd, a, mu=mu, **kw)
+    if op == "tm":
+        kw["b"] = 2 * 0.12195 * mu
+    out = apply_op(Fs, op, be, parity, dagger, din, xd, a, **kw)
     res = reference(Fs, op, parity, dagger, psi, x, a, mu=mu)
     return PR.assert_within(Fs.read(out), res, Fs.prec, what or f"{op} p={parity} dag={dagger} {kind}")
 
@@ -126,17 +117,9 @@ def check_partitioned(Fs, op, be, comm_dim, split=None, parity=0, dagger=1, seed
             ref, T = PR.project_face(psi, Fs.X, 1 - parity, d, 0 if f == 1 else 1, dagger, Fs.prec)
             worst = max(worst, PR.assert_within(h, PR.Result(ref, PR.U_P[Fs.prec] * T), Fs.prec,
                                                 f"ghost d={d} f={f}"))
-    kws = {"tiles": [dict(kernel=4), dict(kernel=3)], "sites": [dict(kernel=6), dict(kernel=5)],
-           "reference": [dict(kernel=1), dict(kernel=2)]}.get(split, [dict()])
     out = Fs.empty()
-    for kw in kws:
-        if op == "wilson":
-            D.ApplyWilson(out, din, Fs.U, a, xd, parity, dagger, halo=halo, backend=be, **kw)
-        elif op == "clover_pc":
-            D.ApplyWilsonCloverPreconditioned(out, din, Fs.U, Fs.inv_field()[0], a, xd, parity, dagger, halo=halo,
-                                              backend=be, **kw)
-        else:
-            D.ApplyWilsonClover(out, din, Fs.U, Fs.Adev, a, xd, parity, dagger, halo=halo, backend=be, **kw)
+    for kw in ops.SPLITS[split]:
+        ops.apply(Fs, op, out, din, a, xd, parity, dagger, halo=halo, backend=be, **kw)
     res = reference(Fs, op, parity, dagger, psi, x, a, ghosts)
     if split == "reference" and Fs.prec == 2 and op == "wilson":
         # the interior kernel stores the partial sum x + a D_interior in the half output and the exterior kernel reads
@@ -157,18 +140,13 @@ def check_multi(Fs, op, be, n_src, parity=1, dagger=0, xpay=True, seed=50, **kw)
         d, p = Fs.spinor(PR.gaussian_spinor(Fs.X, seed + 100 + i))
         xs.append(d)
         xv.append(p)
-    a = -0.12195 if xpay or op == "clover" else 0.0
+    with_x = ops.takes_x(op, xpay)
+    a = -0.12195 if with_x else 0.0
     outs = [Fs.empty() for _ in range(n_src)]
-    xl = xs if (xpay or op == "clover") else None
-    if op == "wilson":
-        D.ApplyWilson(outs, ins, Fs.U, a, xl, parity, dagger, backend=be, **kw)
-    elif op == "clover_pc":
-        D.ApplyWilsonCloverPreconditioned(outs, ins, Fs.U, Fs.inv_field()[0], a, xl, parity, dagger, backend=be, **kw)
-    else:
-        D.ApplyWilsonClover(outs, ins, Fs.U, Fs.Adev, a, xl, parity, dagger, backend=be, **kw)
+    ops.apply(Fs, op, outs, ins, a, xs if with_x else None, parity, dagger, backend=be, **kw)
     worst = 0.0
     for i in range(n_src):
-        res = reference(Fs, op, parity, dagger, psis[i], xv[i] if xl else None, a)
+        res = reference(Fs, op, parity, dagger, psis[i], xv[i] if with_x else None, a)
         worst = max(worst, PR.assert_within(Fs.read(outs[i]), res, Fs.prec, f"multi-RHS {op} source {i}/{n_src}"))
     return worst
 
@@ -177,12 +155,12 @@ def check_clover_apply(Fs, be, inverse, parity=1, seed=21, kind="gauss"):
     din, psi = Fs.spinor(spinor_kind(Fs.X, kind, seed, Fs.prec))
     out = Fs.empty()
     if inverse:
-        dev, dec = Fs.inv_field()
-        D.ApplyClover(out, din, dev, True, parity, backend=be)
-        res = PR.clover_apply(dec, psi, parity, True, Fs.dynamic, Fs.prec)
+        field = ops.clover_inverse(Fs)
+        D.ApplyClover(out, din, field, True, parity, backend=be)
+        res = PR.clover_apply(Fs.image[field], psi, parity, True, Fs.dynamic, Fs.prec)
     else:
-        D.ApplyClover(out, din, Fs.Adev, False, parity, backend=be)
-        res = PR.clover_apply(Fs.A, psi, parity, False, True, Fs.prec)
+        D.ApplyClover(out, din, Fs.A, False, parity, backend=be)
+        res = PR.clover_apply(Fs.image[Fs.A], psi, parity, False, True, Fs.prec)
     return PR.assert_within(Fs.read(out), res, Fs.prec, f"ApplyClover inverse={inverse} {kind}")
 
 

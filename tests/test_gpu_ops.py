@@ -1,6 +1,7 @@
-"""GPU tier: the operator-level cases of tests/ops.py through libquda_b200.so -- xpay / dagger / full fields,
-clover variants, and the self-partitioned halo path (pack kernel -> ghost buffers + arrival flags -> interior +
-fused exterior kernel) for the partition masks dslash_ctest uses (tests/dslash_ctest.cpp:40-42,174-186)."""
+"""GPU tier: the case bodies of tests/ops.py (ops.check_*, which the CPU tier runs on the host twin) through
+libquda_b200.so -- xpay / dagger / full fields, clover variants, multi-RHS batches, twisted mass and the
+self-partitioned halo path (pack kernel -> ghost buffers -> interior + fused exterior kernel) for the partition masks
+dslash_ctest uses (tests/dslash_ctest.cpp:40-42,174-186) -- plus the self exchange with arrival flags."""
 import numpy as np
 import pytest
 

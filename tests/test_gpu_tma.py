@@ -1,7 +1,6 @@
 """GPU tier (-m gpu): the TMA-staged marching kernel (quda_b200/csrc/tma_kernel.cuh: cp.async.bulk.tensor box loads,
 mbarrier producer/consumer pipeline) through the C ABI against the CPU oracle.  B200_TMA=2 makes the library fail
 instead of silently falling back to the gather kernel, so every case below is a real TMA launch."""
-import numpy as np
 import pytest
 
 import ops
@@ -29,76 +28,32 @@ def tma(monkeypatch):
                                           ((8, 6, 10, 4), 8, 8), ((48, 2, 2, 4), 4, 12), ((16, 16, 16, 16), 4, 12),
                                           ((16, 16, 16, 16), 8, 12)])
 def test_tma_wilson_dslash(tma, X, prec, recon):
-    P = Problem(X, prec, recon, CudaMem)
-    for parity in (0, 1):
-        for dagger in (0, 1):
-            s = P.spinor(seed=11 + parity)
-            out = P.empty()
-            D.ApplyWilson(out, P.to_dev(s), P.U, 0.0, None, parity, dagger)
-            ref = oracle.wil_dslash(P.gauge, s, X, parity, dagger)
-            dev = assert_close(ref, P.to_host(out), prec, recon, f"X={X} parity={parity} dagger={dagger}")
-            if prec == 8:
-                assert dev <= 1e-12
+    dev = ops.check_wilson_dslash(CudaMem, None, prec, recon, X)
+    if prec == 8:
+        assert dev <= 1e-12
 
 
 @pytest.mark.parametrize("links", [-1, 0, 2, 3, 4])
 @pytest.mark.parametrize("grid", [1, 3, 37, 148, 1000])
 def test_tma_pipeline_depths_and_work_ranges(tma, links, grid):
-    """both link modes (-1: register stream, 0 / n: shared-memory stages) and every work partition (ranges that start / end
-    mid-tile, one item per CTA, one CTA for everything): no deadlock, no slot hazard, every site visited once"""
-    tma.setenv("B200_TMA_LINKS", str(links))
-    tma.setenv("B200_TMA_GRID", str(grid))
-    X = (16, 4, 8, 6)
-    P = Problem(X, 4, 12, CudaMem, anisotropy=1.7)
-    s = P.spinor(seed=5)
-    out = P.empty()
-    D.ApplyWilson(out, P.to_dev(s), P.U, 0.0, None, 1, 0)
-    assert_close(oracle.wil_dslash(P.gauge, s, X, 1, 0), P.to_host(out), 4, 12, f"links={links} grid={grid}")
+    ops.check_tma_work_ranges(CudaMem, None, tma, links, grid)
 
 
 @pytest.mark.parametrize("prefetch", [2, 3, 4])
 @pytest.mark.parametrize("rings", ["4 2", "5 2", "6 3", "8 4"])
 @pytest.mark.parametrize("grid", [5, 148])
 def test_tma_register_stream_links(tma, prefetch, rings, grid):
-    """register-stream links: every prefetch distance (the reload of a direction pair targets this item or the next one)
-    and spinor ring depth, with work ranges that cross tiles and parities (full field)"""
-    tma.setenv("B200_TMA_LINKS", "-1")
-    tma.setenv("B200_TMA_PREFETCH", str(prefetch))
-    tma.setenv("B200_TMA_RINGS", rings)
-    tma.setenv("B200_TMA_GRID", str(grid))
-    X = (8, 4, 4, 6)
-    P = Problem(X, 4, 12, CudaMem)
-    full = P.spinor(seed=3, nparity=2)
-    out = P.empty(2)
-    D.ApplyWilson(out, P.to_dev(full, 2), P.U, 0.0, None, D.QUDA_INVALID_PARITY, 1)
-    ref = np.concatenate([oracle.wil_dslash(P.gauge, full[P.Vh:], X, 0, 1), oracle.wil_dslash(P.gauge, full[:P.Vh], X, 1, 1)])
-    assert_close(ref, P.to_host(out), 4, 12, f"prefetch={prefetch} rings={rings}")
+    ops.check_tma_register_stream_links(CudaMem, None, tma, prefetch, rings, grid)
 
 
 @pytest.mark.parametrize("l2pf", [-1, 1, 2, 5])
 def test_tma_l2_prefetch_lookahead(tma, l2pf):
-    """the L2 prefetch of the link boxes is a hint (no functional effect) but its coordinates come from the same box
-    function: every look-ahead, including one beyond the end of a CTA's work range, must leave the result unchanged"""
-    tma.setenv("B200_TMA_L2PF", str(l2pf))
-    tma.setenv("B200_TMA_GRID", "7")
-    X = (16, 4, 4, 6)
-    P = Problem(X, 4, 12, CudaMem)
-    s = P.spinor(seed=8)
-    out = P.empty()
-    D.ApplyWilson(out, P.to_dev(s), P.U, 0.0, None, 0, 0)
-    assert_close(oracle.wil_dslash(P.gauge, s, X, 0, 0), P.to_host(out), 4, 12, f"l2pf={l2pf}")
+    ops.check_tma_l2_prefetch_lookahead(CudaMem, None, tma, l2pf)
 
 
 @pytest.mark.parametrize("tile", ["1 1", "2 1", "1 2", "4 2", "2 4", "4 4", "8 1"])
 def test_tma_tiles(tma, tile):
-    tma.setenv("B200_TMA_TILE", tile)
-    X = (8, 8, 4, 4)
-    P = Problem(X, 4, 12, CudaMem)
-    s = P.spinor(seed=6)
-    for parity in (0, 1):
-        out = P.empty()
-        D.ApplyWilson(out, P.to_dev(s), P.U, 0.0, None, parity, 1)
-        assert_close(oracle.wil_dslash(P.gauge, s, X, parity, 1), P.to_host(out), 4, 12, f"tile {tile} parity {parity}")
+    ops.check_tma_tiles(CudaMem, None, tma, tile)
 
 
 @pytest.mark.parametrize("prec,recon", [(8, 18), (8, 12), (4, 12), (4, 8)])

@@ -6,6 +6,7 @@ import os
 import numpy as np
 import pytest
 
+import ops
 import oracle
 from common import CudaMem, Problem, assert_close
 from quda_b200 import dslash as D
@@ -31,16 +32,9 @@ def _native_loaded():
 @pytest.mark.parametrize("recon", RECONS)
 @pytest.mark.parametrize("X", [(8, 8, 8, 8), (4, 6, 8, 10)])
 def test_wilson_dslash_vs_oracle(prec, recon, X):
-    P = Problem(X, prec, recon, CudaMem)
-    for parity in (0, 1):
-        for dagger in (0, 1):
-            s = P.spinor(seed=11 + parity)
-            out = P.empty()
-            D.ApplyWilson(out, P.to_dev(s), P.U, 0.0, None, parity, dagger)
-            ref = oracle.wil_dslash(P.gauge, s, X, parity, dagger)
-            dev = assert_close(ref, P.to_host(out), prec, recon, f"dslash parity={parity} dagger={dagger}")
-            if prec == 8:
-                assert dev <= 1e-12
+    dev = ops.check_wilson_dslash(CudaMem, None, prec, recon, X)
+    if prec == 8:
+        assert dev <= 1e-12
 
 
 @pytest.mark.parametrize("prec", PRECS)
@@ -51,7 +45,7 @@ def test_wilson_xpay_and_tiles(prec, recon):
     P = Problem(X, prec, recon, CudaMem, anisotropy=1.7, antiperiodic_t=True)
     kappa = 0.12195
     s, xs = P.spinor(seed=3), P.spinor(seed=4)
-    ref = xs.astype(np.float64) - kappa * oracle.wil_dslash(P.gauge, s, X, 1, 0).astype(np.float64)
+    ref = ops.reference(P, "wilson", s, 1, 0, xs, -kappa)
     for tile in (None, (4, 1, 1, 1), (4, 6, 1, 1), (2, 2, 2, 2), (3, 4, 4, 4), (4, 6, 4, 3)):
         out = P.empty()
         D.ApplyWilson(out, P.to_dev(s), P.U, -kappa, P.to_dev(xs), 1, 0, tile=tile)

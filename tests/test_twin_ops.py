@@ -1,12 +1,16 @@
 """CPU tier: operator-level parity of the product's site code (host twin) against the oracle:
 xpay / dagger / full fields, clover (compressed + dynamic Cholesky, uncompressed + static inverse),
 self-partitioned halo (pack + interior + fused exterior) for all 16 partition masks."""
-import itertools
+import ctypes as C
 
+import numpy as np
 import pytest
 
 import ops
-from common import HostMem, twin_backend
+import oracle
+from common import HostMem, Problem, assert_close, host_self_exchange, twin_backend
+from quda_b200 import comm, dslash as D, fields as F, lib as L
+from quda_b200.lib import B200Error
 
 
 @pytest.mark.parametrize("prec", [8, 4, 2])
@@ -46,7 +50,7 @@ def test_partitioned_clover(op, prec, comm_dim):
 @pytest.mark.parametrize("comm_dim", MASKS)
 def test_partitioned_reference_style_split(comm_dim):
     """explicit INTERIOR (masked partial sums) + EXTERIOR (read-modify-write) kernels, the reference's decomposition"""
-    ops.check_partitioned(HostMem, twin_backend(), 8, 12, comm_dim, X=(4, 6, 4, 8), xpay=True, split=True)
+    ops.check_partitioned(HostMem, twin_backend(), 8, 12, comm_dim, X=(4, 6, 4, 8), xpay=True, split="reference")
 
 
 @pytest.mark.parametrize("op", ["wilson", "clover_pc", "clover"])
@@ -91,9 +95,6 @@ def test_multi_rhs_full_fields_and_fallback():
 
 
 def test_multi_rhs_argument_checks():
-    from common import Problem
-    from quda_b200 import dslash as D
-    from quda_b200.lib import B200Error
     be = twin_backend()
     P = Problem((4, 4, 4, 4), 4, 12, HostMem)
     ins = [P.to_dev(P.spinor(seed=i)) for i in range(3)]
@@ -139,9 +140,6 @@ def test_twisted_mass_partitioned(prec, comm_dim):
 
 
 def test_twisted_mass_argument_checks():
-    from common import Problem
-    from quda_b200 import dslash as D
-    from quda_b200.lib import B200Error
     be = twin_backend()
     P = Problem((4, 4, 4, 4), 4, 12, HostMem)
     s, out = P.to_dev(P.spinor(seed=1)), P.empty()
@@ -212,10 +210,6 @@ def test_batched_halo_batched_interior_flavours(monkeypatch, flavour, prec, reco
 def test_batched_halo_arrival_protocol():
     """the ticket protocol of the batched pack (host-twin CTA walk in scrambled order): every face's arrival counter moves
     exactly once, after all sources have landed, to the value a single exchange `seq` would publish"""
-    import ctypes as C
-    import numpy as np
-    from quda_b200 import dslash as D, fields as F, lib as L
-    from common import Problem
     be = twin_backend()
     X, prec, n_src = (4, 6, 4, 8), 4, 3
     P = Problem(X, prec, 12, HostMem)
@@ -250,9 +244,6 @@ def test_batched_halo_arrival_protocol():
 
 
 def test_batched_halo_argument_checks():
-    import ctypes as C
-    from quda_b200 import lib as L
-    from common import Problem
     be = twin_backend()
     P = Problem((4, 4, 4, 4), 4, 12, HostMem)
     f = P.to_dev(P.spinor())
@@ -276,14 +267,12 @@ def test_batched_halo_argument_checks():
     with pytest.raises(L.B200Error, match="n_src"):
         be.call("pack_ghost_multi", C.byref(a), 0, srcs, ok)
     # a batch on a partitioned lattice needs one ghost slab per source: src_stride 0 (all sources on slab 0) is refused
-    from quda_b200 import dslash as D
-    import ops
     halo = ops.self_halo(P, HostMem, (0, 0, 0, 1))
     outs, ins = [P.empty(), P.empty()], [f, P.to_dev(P.spinor(seed=3))]
     with pytest.raises(L.B200Error, match="own ghost slab"):
         D.ApplyWilson(outs, ins, P.U, 0.0, None, 0, 0, halo=halo, backend=be)
     # the fused Dslash refuses pack arguments that do not describe its own input's faces
-    dst = [[None, None]] * 3 + [[halo.ghost[3][1], halo.ghost[3][0]]]
+    dst = ops.self_targets(halo)
     fused = dict(halo=halo, fused_dst=dst, block_counter=HostMem.empty(32))
 
     def tampered(edit):  # the twin, with the pack arguments edited on the way in
@@ -307,10 +296,6 @@ def test_batched_halo_argument_checks():
 def test_batched_exchange_schedule_with_arrival_counters(prec, recon, n_src, dims):
     """HaloExchange(mode="self", n_src=...) end to end on the CPU stand-in: batched and single exchanges interleaved on the
     same double-buffered slabs; the twin refuses to run a boundary role whose arrival counter is below its target"""
-    import numpy as np
-    import oracle
-    from common import Problem, assert_close, host_self_exchange
-    from quda_b200 import comm
     X = (8, 4, 4, 8)
     P = Problem(X, prec, recon, HostMem)
     ex = host_self_exchange(X, prec, dims, n_src)
@@ -330,8 +315,6 @@ def test_batched_exchange_schedule_with_arrival_counters(prec, recon, n_src, dim
 
 def test_twin_refuses_a_halo_that_never_arrives():
     """negative control of the check above: a Dslash whose exchange number is ahead of the counters is an error"""
-    from common import Problem, host_self_exchange
-    from quda_b200 import comm, dslash as D, lib as L
     X = (4, 4, 4, 8)
     P = Problem(X, 4, 12, HostMem)
     ex = host_self_exchange(X, 4, (0, 0, 0, 1))
@@ -352,9 +335,8 @@ def test_minimal_and_ragged_lattices(X):
     for d in range(4):
         mask = tuple(int(e == d) for e in range(4))
         if X[d] >= 4:
-            for split in (False, "tiles", "sites", "fused", "fused_roles"):
+            for split in (None, "tiles", "sites", "fused", "fused_roles"):
                 ops.check_partitioned(HostMem, be, 4, 12, mask, X=X, xpay=True, split=split)
         else:
-            from quda_b200 import lib as L
             with pytest.raises(L.B200Error, match="needs local extent >= 4"):
                 ops.check_partitioned(HostMem, be, 4, 12, mask, X=X)

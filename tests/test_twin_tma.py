@@ -5,13 +5,10 @@ B200_TMA=2 makes the twin FAIL if the TMA path does not serve the shape, so ever
 emulated pipeline: box loads interpreted from the tensor-map descriptions, producer program replayed against slot
 ownership (overwriting a live slot, reading a released one -- it is poisoned with NaNs -- or a state where neither
 producer nor consumers can advance all fail the test)."""
-import numpy as np
 import pytest
 
 import ops
-import oracle
-from common import HostMem, Problem, assert_close, twin_backend
-from quda_b200 import dslash as D
+from common import HostMem, Problem, twin_backend
 
 
 @pytest.fixture
@@ -24,81 +21,30 @@ def tma(monkeypatch):
                                           ((32, 4, 4, 4), 4, 18), ((16, 4, 8, 4), 8, 12), ((16, 4, 4, 6), 8, 18),
                                           ((8, 6, 10, 4), 8, 8), ((48, 2, 2, 4), 4, 12)])
 def test_tma_wilson_dslash(tma, X, prec, recon):
-    be = twin_backend()
-    P = Problem(X, prec, recon, HostMem)
-    for parity in (0, 1):
-        for dagger in (0, 1):
-            s = P.spinor(seed=11 + parity)
-            out = P.empty()
-            D.ApplyWilson(out, P.to_dev(s), P.U, 0.0, None, parity, dagger, backend=be)
-            ref = oracle.wil_dslash(P.gauge, s, X, parity, dagger)
-            assert_close(ref, P.to_host(out), prec, recon, f"X={X} parity={parity} dagger={dagger}")
+    ops.check_wilson_dslash(HostMem, twin_backend(), prec, recon, X)
 
 
 @pytest.mark.parametrize("links", [-1, 0, 2, 3, 4])
 @pytest.mark.parametrize("grid", [1, 3, 7, 37, 148, 1000])
 def test_tma_pipeline_depths_and_work_ranges(tma, links, grid):
-    """both link modes (-1: register stream, 0 / n: shared-memory stages) and every work partition (ranges that start / end
-    mid-tile, one item per CTA, one CTA for everything): no deadlock, no slot hazard, every site visited once"""
-    tma.setenv("B200_TMA_LINKS", str(links))
-    tma.setenv("B200_TMA_GRID", str(grid))
-    be = twin_backend()
-    X = (16, 4, 8, 6)
-    P = Problem(X, 4, 12, HostMem, anisotropy=1.7)
-    s = P.spinor(seed=5)
-    out = P.empty()
-    D.ApplyWilson(out, P.to_dev(s), P.U, 0.0, None, 1, 0, backend=be)
-    assert_close(oracle.wil_dslash(P.gauge, s, X, 1, 0), P.to_host(out), 4, 12, f"links={links} grid={grid}")
+    ops.check_tma_work_ranges(HostMem, twin_backend(), tma, links, grid)
 
 
 @pytest.mark.parametrize("prefetch", [2, 3, 4])
 @pytest.mark.parametrize("rings", ["4 2", "5 2", "6 3", "8 4"])
 @pytest.mark.parametrize("grid", [5, 148])
 def test_tma_register_stream_links(tma, prefetch, rings, grid):
-    """register-stream links: every prefetch distance (the reload of a direction pair targets this item or the next one)
-    and spinor ring depth, with work ranges that cross tiles and parities (full field)"""
-    tma.setenv("B200_TMA_LINKS", "-1")
-    tma.setenv("B200_TMA_PREFETCH", str(prefetch))
-    tma.setenv("B200_TMA_RINGS", rings)
-    tma.setenv("B200_TMA_GRID", str(grid))
-    be = twin_backend()
-    X = (8, 4, 4, 6)
-    P = Problem(X, 4, 12, HostMem)
-    full = P.spinor(seed=3, nparity=2)
-    out = P.empty(2)
-    D.ApplyWilson(out, P.to_dev(full, 2), P.U, 0.0, None, D.QUDA_INVALID_PARITY, 1, backend=be)
-    ref = np.concatenate([oracle.wil_dslash(P.gauge, full[P.Vh:], X, 0, 1), oracle.wil_dslash(P.gauge, full[:P.Vh], X, 1, 1)])
-    assert_close(ref, P.to_host(out), 4, 12, f"prefetch={prefetch} rings={rings}")
+    ops.check_tma_register_stream_links(HostMem, twin_backend(), tma, prefetch, rings, grid)
 
 
 @pytest.mark.parametrize("l2pf", [-1, 1, 2, 5])
 def test_tma_l2_prefetch_lookahead(tma, l2pf):
-    """the L2 prefetch of the link boxes is a hint (no functional effect) but its coordinates come from the same box
-    function: every look-ahead, including one beyond the end of a CTA's work range, must leave the result unchanged"""
-    tma.setenv("B200_TMA_L2PF", str(l2pf))
-    tma.setenv("B200_TMA_GRID", "7")
-    be = twin_backend()
-    X = (16, 4, 4, 6)
-    P = Problem(X, 4, 12, HostMem)
-    s = P.spinor(seed=8)
-    out = P.empty()
-    D.ApplyWilson(out, P.to_dev(s), P.U, 0.0, None, 0, 0, backend=be)
-    assert_close(oracle.wil_dslash(P.gauge, s, X, 0, 0), P.to_host(out), 4, 12, f"l2pf={l2pf}")
+    ops.check_tma_l2_prefetch_lookahead(HostMem, twin_backend(), tma, l2pf)
 
 
 @pytest.mark.parametrize("tile", ["1 1", "2 1", "1 2", "4 2", "2 4", "4 4", "8 1"])
 def test_tma_tiles(tma, tile):
-    """tile shapes incl. TY == 1 / TZ == 1 (the backward y / z links then come from one box only) and a tile that
-    spans the whole extent (the halo rows are the tile's own opposite edge)"""
-    tma.setenv("B200_TMA_TILE", tile)
-    be = twin_backend()
-    X = (8, 8, 4, 4)
-    P = Problem(X, 4, 12, HostMem)
-    s = P.spinor(seed=6)
-    for parity in (0, 1):
-        out = P.empty()
-        D.ApplyWilson(out, P.to_dev(s), P.U, 0.0, None, parity, 1, backend=be)
-        assert_close(oracle.wil_dslash(P.gauge, s, X, parity, 1), P.to_host(out), 4, 12, f"tile {tile} parity {parity}")
+    ops.check_tma_tiles(HostMem, twin_backend(), tma, tile)
 
 
 @pytest.mark.parametrize("prec,recon", [(8, 18), (8, 12), (4, 12), (4, 8)])
@@ -120,7 +66,4 @@ def test_tma_unserved_shapes_fall_back(monkeypatch):
     be = twin_backend()
     for X, prec, recon in (((4, 4, 4, 4), 2, 12), ((4, 6, 2, 2), 4, 12)):
         P = Problem(X, prec, recon, HostMem)
-        s = P.spinor(seed=2)
-        out = P.empty()
-        D.ApplyWilson(out, P.to_dev(s), P.U, 0.0, None, 0, 0, backend=be)
-        assert_close(oracle.wil_dslash(P.gauge, s, X, 0, 0), P.to_host(out), prec, recon, f"fallback X={X}")
+        ops.wilson_vs_oracle(P, be, P.spinor(seed=2), 0, 0, f"fallback X={X}")

@@ -1,9 +1,8 @@
 """CPU tier: the product's site code (compiled for the host, tests/hosttwin) against the oracle.
 Same b200_dslash_args ABI, same native layouts, same argument validation as the CUDA library."""
-import numpy as np
 import pytest
 
-import oracle
+import ops
 from common import HostMem, Problem, assert_close, twin_backend
 from quda_b200 import dslash as D
 
@@ -15,15 +14,7 @@ RECONS = [18, 12, 8]
 @pytest.mark.parametrize("recon", RECONS)
 @pytest.mark.parametrize("X", [(4, 4, 4, 4), (8, 4, 6, 2)])
 def test_wilson_dslash(prec, recon, X):
-    be = twin_backend()
-    P = Problem(X, prec, recon, HostMem)
-    for parity in (0, 1):
-        for dagger in (0, 1):
-            s = P.spinor(seed=11 + parity)
-            out = P.empty()
-            D.ApplyWilson(out, P.to_dev(s), P.U, 0.0, None, parity, dagger, backend=be)
-            ref = oracle.wil_dslash(P.gauge, s, X, parity, dagger)
-            assert_close(ref, P.to_host(out), prec, recon, f"dslash parity={parity} dagger={dagger}")
+    ops.check_wilson_dslash(HostMem, twin_backend(), prec, recon, X)
 
 
 @pytest.mark.parametrize("tile", [(16, 2, 2, 1), (2, 2, 2, 2), (1, 4, 1, 2), (4, 1, 1, 1), (2, 8, 4, 2), (3, 4, 4, 2)])
@@ -33,15 +24,11 @@ def test_launch_tilings_cover_the_lattice(tile):
     be = twin_backend()
     X = (8, 6, 4, 6)
     P = Problem(X, 4, 12, HostMem)
-    s = P.spinor(seed=2)
-    out = P.empty()
-    D.ApplyWilson(out, P.to_dev(s), P.U, 0.0, None, 1, 0, tile=tile, backend=be)
-    assert_close(oracle.wil_dslash(P.gauge, s, X, 1, 0), P.to_host(out), 4, 12, f"tile {tile}")
+    ops.wilson_vs_oracle(P, be, P.spinor(seed=2), 1, 0, f"tile {tile}", tile=tile)
     full = P.spinor(seed=3, nparity=2)
     out2 = P.empty(2)
     D.ApplyWilson(out2, P.to_dev(full, 2), P.U, 0.0, None, D.QUDA_INVALID_PARITY, 0, tile=tile, backend=be)
-    ref = np.concatenate([oracle.wil_dslash(P.gauge, full[P.Vh:], X, 0, 0), oracle.wil_dslash(P.gauge, full[:P.Vh], X, 1, 0)])
-    assert_close(ref, P.to_host(out2), 4, 12, f"full-field tile {tile}")
+    assert_close(ops.full_dslash(P, full, 0), P.to_host(out2), 4, 12, f"full-field tile {tile}")
 
 
 @pytest.mark.parametrize("X", [(2, 2, 2, 2), (2, 4, 2, 6), (4, 2, 2, 2), (16, 2, 4, 2)])
@@ -55,5 +42,4 @@ def test_degenerate_extents(X, prec, recon):
         s, xs = P.spinor(seed=7 + parity), P.spinor(seed=9)
         out = P.empty()
         D.ApplyWilson(out, P.to_dev(s), P.U, -0.1, P.to_dev(xs), parity, dagger, backend=be)
-        ref = xs.astype(np.float64) - 0.1 * oracle.wil_dslash(P.gauge, s, X, parity, dagger).astype(np.float64)
-        assert_close(ref, P.to_host(out), prec, recon, f"X={X} parity={parity}")
+        assert_close(ops.reference(P, "wilson", s, parity, dagger, xs, -0.1), P.to_host(out), prec, recon, f"X={X} parity={parity}")
