@@ -239,6 +239,18 @@ int b200_copy_gauge(const b200_gauge *native, int native_precision, const int X[
 int b200_copy_clover(const b200_clover *native, int native_precision, const int X[4], const void *packed, int host_precision,
                      void *stream);
 
+/* The clover term computed from the links (loadCloverQuda with compute_clover, lib/interface_quda.cpp:803-900):
+ * packed[V][2][36] = A = 1 + coeff sum_{mu<nu} sigma_mu,nu F_mu,nu (clover-leaf F, both chiral blocks, packed order as
+ * b200_copy_clover reads it), coeff = kappa * c_sw (QudaInvertParam::clover_coeff).  qdp[mu] are device QDP-order links
+ * [2 Vh_e][3][3][2] of the extended lattice X_e = X + 2 border: border[d] = 0 wraps periodically inside the local block,
+ * border[d] = 1 means the caller filled a depth-1 halo, corners included.  precision (8 or 4) is that of links and output. */
+int b200_compute_clover(void *packed, const void *const qdp[4], const int X[4], const int border[4],
+                        int precision /* 8 or 4: links and output */, double coeff, void *stream);
+/* packed_inv = A^-1 by Cholesky in double (NULL: trlog only); trlog[p] = sum over parity-p sites and both chiralities of
+ * log det A (a host array).  The sums are taken in a fixed order, so repeated calls give bit-identical values.
+ * Synchronises the stream, as cloverInvert does for its reduction. */
+int b200_clover_invert_packed(void *packed_inv, double trlog[2], const void *packed, const int X[4], int precision, void *stream);
+
 /* Halo buffers that peer GPUs must be able to map: plain cudaMalloc allocations (zero-filled) plus CUDA-IPC
  * export / import.  Replaces the reference's static ghost buffers + IPC handle exchange
  * (lib/lattice_field.cpp:252-470, lib/targets/cuda/comm_target.cpp:37-167); the 64-byte handles travel between

@@ -105,6 +105,50 @@ def local_slice(global_field, Xg, Xl, coords, kind):
     raise ValueError(kind)
 
 
+def _lex_of_sites(X):
+    """lexicographic index ((t X2 + z) X1 + y) X0 + x of every parity-major QDP site"""
+    c = np.concatenate([F.cb_coords(X, p) for p in range(2)])
+    return ((c[:, 3] * X[2] + c[:, 2]) * X[1] + c[:, 1]) * X[0] + c[:, 0]
+
+
+def extend_gauge(grid, gauge_local, X, dist):
+    """The local QDP-order links ([4][V][3][3][2], numpy or torch) extended by a depth-1 halo in every partitioned dimension
+    of `grid`: QDP order on X_e = X + 2 comm_dim (parity of the extended coordinates), the lattice the clover kernels read
+    with border = comm_dim (createExtendedGauge with R = 1, lib/gauge_field.cpp / lib/copy_gauge_extended.cu).  Dimension by
+    dimension, each rank sends its first and last interior slabs of the already-extended array to its neighbours, so the
+    halos of earlier dimensions travel along and corners arrive.  torch.distributed send / recv: gloo on the host, NCCL on
+    GPUs (tensors on the device).  Returns the same kind of array as it was given."""
+    import torch
+    is_np = isinstance(gauge_local, np.ndarray)
+    g = torch.from_numpy(np.ascontiguousarray(gauge_local)) if is_np else gauge_local
+    X = [int(v) for v in X]
+    border = grid.comm_dim()
+    Xe = [X[d] + 2 * border[d] for d in range(4)]
+    tail = tuple(g.shape[2:])
+    lex = torch.empty((4, X[0] * X[1] * X[2] * X[3]) + tail, dtype=g.dtype, device=g.device)
+    lex[:, torch.from_numpy(_lex_of_sites(X)).to(g.device)] = g
+    ext = torch.zeros((4, Xe[3], Xe[2], Xe[1], Xe[0]) + tail, dtype=g.dtype, device=g.device)
+    ext[:, border[3]:border[3] + X[3], border[2]:border[2] + X[2], border[1]:border[1] + X[1], border[0]:border[0] + X[0]] = \
+        lex.reshape((4, X[3], X[2], X[1], X[0]) + tail)
+    for d in range(4):
+        if not border[d]:
+            continue
+        ax = 4 - d
+        lo, hi = ext.narrow(ax, 1, 1).contiguous(), ext.narrow(ax, X[d], 1).contiguous()
+        into_hi, into_lo = torch.empty_like(lo), torch.empty_like(hi)
+        bwd, fwd = grid.neighbor(d, -1), grid.neighbor(d, +1)
+        # my first slab is the backward neighbour's upper halo, my last one the forward neighbour's lower halo; with the
+        # same peer on both sides, the sends and the receives pair up in posting order
+        ops = [dist.P2POp(dist.isend, lo, bwd, tag=2 * d), dist.P2POp(dist.isend, hi, fwd, tag=2 * d + 1),
+               dist.P2POp(dist.irecv, into_hi, fwd, tag=2 * d), dist.P2POp(dist.irecv, into_lo, bwd, tag=2 * d + 1)]
+        for req in dist.batch_isend_irecv(ops):
+            req.wait()
+        ext.narrow(ax, Xe[d] - 1, 1).copy_(into_hi)
+        ext.narrow(ax, 0, 1).copy_(into_lo)
+    out = ext.reshape((4, Xe[0] * Xe[1] * Xe[2] * Xe[3]) + tail)[:, torch.from_numpy(_lex_of_sites(Xe)).to(g.device)]
+    return out.contiguous().numpy() if is_np else out.contiguous()
+
+
 class HaloExchange:
     """Ghost buffers + neighbour wiring for one (lattice, precision, site-subset).  Owns its buffers (allocated once,
     like the reference's static ghost buffers, lib/lattice_field.cpp:274-303)."""

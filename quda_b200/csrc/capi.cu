@@ -4,6 +4,7 @@
 #include <cstdlib>
 #include <cstring>
 
+#include "clover_build.h"
 #include "plan.h"
 
 namespace b200
@@ -50,6 +51,8 @@ namespace b200
     template <class P> static int twist(const TwistRequest &rq) { return launch_twist_precision<P>(rq); }
     template <class P> static int pack(const PackRequest &rq) { return launch_pack_precision<P>(rq); }
     template <class P> static int pack_multi(const PackRequest &rq, const PackBatchRequest &b) { return launch_pack_multi_precision<P>(rq, b); }
+    template <typename T> static int clover_build(const CloverBuildRequest &rq) { return launch_clover_build<T>(rq); }
+    template <typename T> static int clover_invert(const CloverInvertRequest &rq) { return launch_clover_invert<T>(rq); }
   };
 
 } // namespace b200
@@ -161,6 +164,17 @@ int b200_copy_clover(const b200_clover *native, int native_precision, const int 
   case B200_HALF: return launch_clover_copy_precision<PrecH16>(rq);
   }
   return set_error(B200_ERR_INVALID, "precision %d not in {8,4,2}", native_precision);
+}
+
+int b200_compute_clover(void *packed, const void *const qdp[4], const int X[4], const int border[4], int precision, double coeff,
+                        void *stream)
+{
+  return compute_clover<Cuda>(packed, qdp, X, border, precision, coeff, stream);
+}
+
+int b200_clover_invert_packed(void *packed_inv, double trlog[2], const void *packed, const int X[4], int precision, void *stream)
+{
+  return clover_invert_packed<Cuda>(packed_inv, trlog, packed, X, precision, stream);
 }
 
 int b200_comm_alloc(void **ptr, size_t bytes)

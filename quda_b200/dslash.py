@@ -288,31 +288,99 @@ def load_gauge(host_gauge, X, prec, recon, anisotropy=1.0, t_boundary=1, ghost_l
     return U
 
 
+def clover_scale(packed, compressed):
+    """(diagonal, max_element) of the native field b200_copy_clover makes from a packed clover [V][2][36] (numpy array or
+    torch tensor, evaluated where it lives): the compressed format stores the diagonals as deviations from `diagonal`, and
+    max_element is twice the largest stored |value| (CloverField::max_element, clover_field_order.h:621-624)."""
+    c = packed.reshape(-1, 36)
+    diagonal = float((0.25 * (c[:, 0:3] + c[:, 3:6])).mean()) if compressed else 0.0
+    half = 0.5 * (c.double() if hasattr(c, "double") else c.astype(np.float64))
+    if compressed:
+        mx = max(abs(half[:, 0:3] - diagonal).max(), abs(half[:, 6:30]).max())
+    else:
+        mx = abs(half).max()
+    return diagonal, 2.0 * float(mx)
+
+
+def _resident_clover(packed_dev, X, prec, compressed, dynamic, diagonal, max_element, stream):
+    """packed device clover -> native CloverField at `prec` (b200_copy_clover)"""
+    import torch
+    lib = L.load()
+    CB = 28 if compressed else 36
+    nbytes = 2 * 2 * CB * F.volume_cb(X) * prec
+    buf = torch.zeros(nbytes, dtype=torch.uint8, device="cuda")
+    meta = dict(parity_stride_bytes=nbytes // 2, diagonal=diagonal, max_element=max_element, compressed=int(compressed))
+    A = CloverField(buf, X, prec, meta, dynamic=dynamic)
+    d = A.desc()
+    Xc = (C.c_int * 4)(*[int(v) for v in X])
+    L.check(lib.b200_copy_clover(C.byref(d), prec, Xc, packed_dev.data_ptr(), packed_dev.element_size(), stream))
+    torch.cuda.synchronize()
+    return A
+
+
 def load_clover(host_clover, X, prec, compressed=True, dynamic=True, stream=None):
     """loadCloverQuda's device work: packed host clover (numpy [V][2][36]) -> resident native CloverField.
     Reference: lib/interface_quda.cpp:804-923, lib/copy_clover.cu."""
     import torch
-    lib = L.load()
-    Vh = F.volume_cb(X)
-    c = np.asarray(host_clover).reshape(-1, 36)
-    diagonal = float(np.mean(0.25 * (c[:, 0:3] + c[:, 3:6]))) if compressed else 0.0
-    CB = 28 if compressed else 36
-    # max |stored value| x 2 (CloverField::max_element convention, clover_field_order.h:621-624)
-    half = 0.5 * c.astype(np.float64)
-    if compressed:
-        mx = max(np.abs(half[:, 0:3] - diagonal).max(), np.abs(half[:, 6:30]).max())
-    else:
-        mx = np.abs(half).max()
-    nbytes = 2 * 2 * CB * Vh * prec
-    buf = torch.zeros(nbytes, dtype=torch.uint8, device="cuda")
-    meta = dict(parity_stride_bytes=nbytes // 2, diagonal=diagonal, max_element=2.0 * float(mx), compressed=int(compressed))
-    A = CloverField(buf, X, prec, meta, dynamic=dynamic)
-    d = A.desc()
+    diagonal, max_element = clover_scale(np.asarray(host_clover), compressed)
     h = torch.from_numpy(np.ascontiguousarray(host_clover)).cuda()
-    Xc = (C.c_int * 4)(*[int(v) for v in X])
-    L.check(lib.b200_copy_clover(C.byref(d), prec, Xc, h.data_ptr(), host_clover.dtype.itemsize, stream))
-    torch.cuda.synchronize()
-    return A
+    return _resident_clover(h, X, prec, compressed, dynamic, diagonal, max_element, stream)
+
+
+def _Xc(X):
+    return (C.c_int * 4)(*[int(v) for v in X])
+
+
+def compute_clover(packed, qdp, X, border, precision, coeff, stream=None, backend=None):
+    """packed [V][2][36] = A = 1 + coeff sum sigma F (clover-leaf F) from the QDP-order links qdp ([4][V_e][3][3][2], or four
+    per-direction buffers) of the lattice X extended by border[d] in {0, 1} sites per side; fp64 (precision 8) or fp32 (4).
+    Reference: lib/interface_quda.cpp:4040-4078 (computeFmunu + computeClover)."""
+    be = backend or cuda_backend()
+    q = (C.c_void_p * 4)(*[_ptr(qdp[mu]) for mu in range(4)])
+    be.call("compute_clover", _ptr(packed), q, _Xc(X), _Xc(border), int(precision), float(coeff), stream)
+
+
+def clover_invert(inv, packed, X, precision, stream=None, backend=None):
+    """inv = A^-1 (inv None: none) of a packed clover by Cholesky; returns [tr log A on even sites, on odd sites].
+    Synchronises `stream`.  Reference: lib/clover_invert.cu, include/kernels/clover_invert.cuh."""
+    be = backend or cuda_backend()
+    tl = (C.c_double * 2)()
+    be.call("clover_invert_packed", _ptr(inv), tl, _ptr(packed), _Xc(X), int(precision), stream)
+    return [tl[0], tl[1]]
+
+
+def compute_clover_field(gauge, X, prec, kappa, csw, compressed=True, dynamic=True, grid=None, dist=None, anisotropy=1.0,
+                         stream=None):
+    """loadCloverQuda(compute_clover=1, compute_clover_inverse=!dynamic): the clover term of the QDP-order links `gauge`
+    ([4][V][3][3][2] of the local lattice X, numpy or torch, fp64 / fp32) with coeff = kappa * csw, computed on the device
+    in fp64 (prec 8) or fp32 (prec 4, 2).  Returns (A, A^-1 or None, trlog) as resident CloverFields at `prec`; the static
+    inverse is stored uncompressed.  With `dist` (torch.distributed) the lattice is the block of `grid` (comm.ProcessGrid):
+    the links of the partitioned dimensions are extended by a depth-1 halo (comm.extend_gauge) and trlog is all-reduced.
+    Reference: lib/interface_quda.cpp:803-900, 4040-4078."""
+    import torch
+    if anisotropy != 1.0:
+        raise L.B200Error("cannot compute anisotropic clover field")
+    hp = F.DOUBLE if prec == F.DOUBLE else F.SINGLE
+    dt = torch.float64 if hp == F.DOUBLE else torch.float32
+    g = torch.as_tensor(gauge).to(device="cuda", dtype=dt).contiguous()
+    border = [0, 0, 0, 0]
+    if dist is not None:
+        from . import comm
+        g = comm.extend_gauge(grid, g, X, dist)
+        border = grid.comm_dim()
+    packed = torch.empty((2 * F.volume_cb(X), 2, 36), dtype=dt, device="cuda")
+    compute_clover(packed, g, X, border, hp, kappa * csw, stream)
+    packed_inv = None if dynamic else torch.empty_like(packed)
+    trlog = clover_invert(packed_inv, packed, X, hp, stream)
+    if dist is not None:
+        t = torch.tensor(trlog, dtype=torch.float64, device="cuda" if dist.get_backend() == "nccl" else "cpu")
+        dist.all_reduce(t)
+        trlog = [float(v) for v in t.cpu()]
+    A = _resident_clover(packed, X, prec, compressed, dynamic, *clover_scale(packed, compressed), stream)
+    Ainv = None
+    if not dynamic:
+        Ainv = _resident_clover(packed_inv, X, prec, False, False, *clover_scale(packed_inv, False), stream)
+    return A, Ainv, trlog
 
 
 def flops_per_site(op=L.OP_WILSON, xpay=False):

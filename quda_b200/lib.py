@@ -118,6 +118,19 @@ def declare(lib, prefix="b200"):
     return lib
 
 
+def declare_clover(lib, prefix="b200"):
+    """Attach argtypes/restypes for the clover construction, shared by the CUDA library and its test-only twin."""
+    f = getattr(lib, prefix + "_compute_clover")
+    f.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int, C.c_double, C.c_void_p]
+    f.restype = C.c_int
+    f = getattr(lib, prefix + "_clover_invert_packed")
+    f.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.c_void_p, C.POINTER(C.c_int), C.c_int, C.c_void_p]
+    f.restype = C.c_int
+    f = getattr(lib, prefix + "_last_error")
+    f.argtypes, f.restype = [], C.c_char_p
+    return lib
+
+
 _lib = None
 
 
@@ -129,6 +142,7 @@ def load():
             raise B200Error(f"{LIB_PATH} not built -- the engine has no fallback path; run __graft_entry__.build()")
         lib = C.CDLL(LIB_PATH)
         declare(lib)
+        declare_clover(lib)
         lib.b200_abi_version.restype = C.c_int
         lib.b200_launch_count.restype = C.c_long
         lib.b200_ghost_face_bytes.argtypes = [C.c_int, C.POINTER(C.c_int), C.c_int]
@@ -183,7 +197,7 @@ def check(rc, lib=None, prefix="b200"):
 
 
 EXPORTED_SYMBOLS = ["b200_dslash_apply", "b200_dslash_apply_fused", "b200_dslash_apply_multi", "b200_clover_apply", "b200_twist_gamma5", "b200_pack_ghost", "b200_pack_ghost_multi", "b200_ghost_face_bytes",
-                    "b200_copy_spinor", "b200_copy_gauge", "b200_copy_clover", "b200_comm_alloc", "b200_comm_free", "b200_ipc_get_handle", "b200_ipc_open_handle",
+                    "b200_copy_spinor", "b200_copy_gauge", "b200_copy_clover", "b200_compute_clover", "b200_clover_invert_packed", "b200_comm_alloc", "b200_comm_free", "b200_ipc_get_handle", "b200_ipc_open_handle",
                     "b200_ipc_close_handle", "b200_comm_copy",
                     "b200_dirac_create", "b200_dirac_set_twist", "b200_dirac_destroy", "b200_dirac_apply", "b200_dirac_prepare",
                     "b200_dirac_reconstruct", "b200_invert_cg", "b200_invert_bicgstab", "b200_invert_multishift_cg",
