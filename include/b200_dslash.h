@@ -363,6 +363,35 @@ typedef struct {
 int b200_invert_multishift_cg(b200_dirac *precise, b200_dirac *sloppy, const b200_spinor *x, const b200_spinor *b,
                               b200_multishift_param *param);
 
+/* The clover fermion force (computeCloverForceQuda -> computeCloverForce, lib/interface_quda.cpp:4539-4612,
+ * lib/clover_force.cpp): non-twisted Wilson-clover, asymmetric even-odd preconditioning, MATPCDAG_MATPC solutions, no
+ * determinant ratio, one GPU (no partitioned dimension).
+ *
+ * Kernel level.  mom[V][4][10] (parity-major sites; per link the (01), (02), (12) complex entries, the three imaginary
+ * diagonals and one pad real, the reference's QUDA_ASQTAD_MOM_LINKS order) is updated in place:
+ *   mom -= TA( U_mu(x) sum_i force_coeff[i] tr_spin[(1+g_mu) x_i(x+mu) p_i(x)^+ + (1-g_mu) p_i(x+mu) x_i(x)^+]
+ *            + clover derivative of oprod ),
+ *   oprod_mu,nu = sum_i epsilon[i][parity] (R_i - R_i^+), R_i = tr_spin[sigma_nu,mu x_i p_i^+],
+ *                 plus sigma_coeff tr_spin[sigma_mu,nu A^-1] on the sites of parity trlog_parity,
+ * TA = traceless anti-Hermitian part.  x[i], p[i] are full-lattice (both parities) native spinors, 1 <= n <=
+ * B200_MAX_SHIFTS; qdp[mu] are the device QDP-order links [V][3][3][2] (boundary signs included, as b200_compute_clover
+ * takes them); packed is A [V][2][36] as b200_compute_clover writes it.  Everything is in `precision` (8 or 4).
+ * Asynchronous on `stream`. */
+int b200_clover_force_accumulate(void *mom, const void *const qdp[4], const void *packed, const int X[4], int precision, int n,
+                                 const void *const *x, const void *const *p, const double *force_coeff,
+                                 const double *epsilon /* [n][2] */, double sigma_coeff, int trlog_parity, void *stream);
+/* Operator level, the arguments of computeCloverForceQuda: mom as above, x[i] the n single-parity solutions (of the
+ * operator's parity) of (Mhat^+ Mhat + sigma_i) x_i = phi as b200_invert_multishift_cg writes them, coeff[i] their residues,
+ * kappa2 = -kappa^2 and ck = -c_sw kappa / 8 as MILC passes them, qdp and packed as above.  op must be a "cloverpc"
+ * operator with asymmetric matpc on an unpartitioned lattice (B200_ERR_INVALID otherwise).  It prepares p_i and the other
+ * parity of x_i on the operator's stream in scratch fields, along the reference's dagger branch (for these solutions the
+ * non-dagger branch is the force of the Mhat Mhat^+ action), then adds the force with force_coeff = 2 dt coeff kappa2,
+ * epsilon = 2 ck coeff dt on the operator's parity and -kappa2 2 ck coeff dt on the other, and sigma_coeff =
+ * 2 ck multiplicity dt on the other parity: the update is the derivative of
+ * sum_i coeff_i phi^+ (Mhat^+ Mhat + sigma_i)^-1 phi - multiplicity tr log A_other.  Synchronises the operator's stream. */
+int b200_clover_force(void *mom, double dt, const b200_spinor *x, const double *coeff, double kappa2, double ck, int n,
+                      double multiplicity, const void *const qdp[4], const void *packed, b200_dirac *op);
+
 const char *b200_last_error(void);
 int b200_abi_version(void);
 /* number of kernels this library has launched since load (bench.py's gpu_launches evidence) */

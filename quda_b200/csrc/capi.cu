@@ -5,6 +5,7 @@
 #include <cstring>
 
 #include "clover_build.h"
+#include "clover_force.h"
 #include "plan.h"
 
 namespace b200
@@ -53,6 +54,7 @@ namespace b200
     template <class P> static int pack_multi(const PackRequest &rq, const PackBatchRequest &b) { return launch_pack_multi_precision<P>(rq, b); }
     template <typename T> static int clover_build(const CloverBuildRequest &rq) { return launch_clover_build<T>(rq); }
     template <typename T> static int clover_invert(const CloverInvertRequest &rq) { return launch_clover_invert<T>(rq); }
+    template <typename T> static int clover_force(const CloverForceRequest &rq) { return launch_clover_force<T>(rq); }
   };
 
 } // namespace b200
@@ -175,6 +177,13 @@ int b200_compute_clover(void *packed, const void *const qdp[4], const int X[4], 
 int b200_clover_invert_packed(void *packed_inv, double trlog[2], const void *packed, const int X[4], int precision, void *stream)
 {
   return clover_invert_packed<Cuda>(packed_inv, trlog, packed, X, precision, stream);
+}
+
+int b200_clover_force_accumulate(void *mom, const void *const qdp[4], const void *packed, const int X[4], int precision, int n,
+                                 const void *const *x, const void *const *p, const double *force_coeff, const double *epsilon,
+                                 double sigma_coeff, int trlog_parity, void *stream)
+{
+  return clover_force_accumulate<Cuda>(mom, qdp, packed, X, precision, n, x, p, force_coeff, epsilon, sigma_coeff, trlog_parity, stream);
 }
 
 int b200_comm_alloc(void **ptr, size_t bytes)

@@ -98,10 +98,10 @@ namespace b200
     a.k = (T)(rq.coeff * 0.125);
   }
 
-  // U_mu at extended-lattice coordinates y + (dmu along mu) + (dnu along nu), wrapped periodically on the extended lattice
-  // (border 0: the local block is periodic; border 1: the shift never leaves the halo)
-  template <typename T>
-  B2_HD void load_link_ext(T *u, const CloverBuildArgs<T> &a, int dir, const int *y, int mu, int dmu, int nu, int dnu)
+  // Parity-major site index (parity Vh_e + x_cb) of extended-lattice coordinates y + (dmu along mu) + (dnu along nu),
+  // wrapped periodically on the extended lattice (border 0: the local block is periodic; border 1: the shift never leaves
+  // the halo)
+  template <typename T> B2_HD size_t site_ext(const CloverBuildArgs<T> &a, const int *y, int mu, int dmu, int nu, int dnu)
   {
     int idx = 0, par = 0;
 #pragma unroll
@@ -111,14 +111,29 @@ namespace b200
       idx = idx * a.Xe[d] + c;
       par += c;
     }
+    return (size_t)(par & 1) * a.volume_cb_e + (idx >> 1);
+  }
+
+  // 3x3 complex matrix of a QDP-order field [2 Vh_e][3][3][2] (a link direction, or one plane of a tensor field) at
+  // site_ext(a, y, mu, dmu, nu, dnu)
+  template <typename T>
+  B2_HD void load_matrix_ext(T *u, const T *field, const CloverBuildArgs<T> &a, const int *y, int mu, int dmu, int nu, int dnu)
+  {
     using V = std::conditional_t<sizeof(T) == 8, d2, f2>;
-    const V *p = reinterpret_cast<const V *>(a.u[dir] + ((size_t)(par & 1) * a.volume_cb_e + (idx >> 1)) * 18);
+    const V *p = reinterpret_cast<const V *>(field + site_ext(a, y, mu, dmu, nu, dnu) * 18);
 #pragma unroll
     for (int i = 0; i < 9; i++) {
       const V w = ld<Cache::REUSE>(p + i);
       u[2 * i] = w.x;
       u[2 * i + 1] = w.y;
     }
+  }
+
+  // U_dir at site_ext(a, y, mu, dmu, nu, dnu)
+  template <typename T>
+  B2_HD void load_link_ext(T *u, const CloverBuildArgs<T> &a, int dir, const int *y, int mu, int dmu, int nu, int dnu)
+  {
+    load_matrix_ext(u, a.u[dir], a, y, mu, dmu, nu, dnu);
   }
 
   // r = op(a) op(b) (acc: r += op(a) op(b)) for 3x3 complex matrices [3][3][2]; op = dagger where the flag is set

@@ -1137,6 +1137,33 @@ namespace b200
         });
       }
       void zero(ColorSpinorField &x, const Exec &ex) { cuda_ok(cudaMemsetAsync(x.v, 0, x.Bytes(), cs(ex.stream)), "memset"); }
+
+      // gamma5 in the UKQCD basis swaps spins (0, 1) with (2, 3): the first 12 reals of a site with the last 12, which in
+      // the native order (fp64: 2 reals per 16-byte plane, fp32: 4) is the first half of the planes with the second half
+      __global__ void gamma5_kernel(const uint4 *__restrict__ in, uint4 *__restrict__ out, int volume_cb, int half_planes,
+                                    size_t parity_elems)
+      {
+        const int x = blockIdx.x * blockDim.x + threadIdx.x;
+        if (x >= volume_cb) return;
+        const uint4 *i = in + blockIdx.y * parity_elems;
+        uint4 *o = out + blockIdx.y * parity_elems;
+        for (int k = 0; k < half_planes; k++) {
+          const uint4 a = i[(size_t)k * volume_cb + x], b = i[(size_t)(k + half_planes) * volume_cb + x];
+          o[(size_t)k * volume_cb + x] = b;
+          o[(size_t)(k + half_planes) * volume_cb + x] = a;
+        }
+      }
+
+      void gamma5(ColorSpinorField &out, const ColorSpinorField &in, const Exec &ex)
+      {
+        check_pair(in, out);
+        if (out.n_parity != in.n_parity) throw Error("blas::gamma5: fields cover different site subsets");
+        if (in.precision != B200_DOUBLE && in.precision != B200_SINGLE) throw Error("blas::gamma5: precision must be 8 or 4");
+        const int vcb = in.VolumeCB(), planes = 24 * in.precision / 16;
+        gamma5_kernel<<<dim3((vcb + 127) / 128, in.n_parity), 128, 0, cs(ex.stream)>>>(
+          static_cast<const uint4 *>(in.v), static_cast<uint4 *>(out.v), vcb, planes / 2, (size_t)planes * vcb);
+        cuda_ok(cudaGetLastError(), "gamma5 launch");
+      }
       void axpy(double a, const ColorSpinorField &x, ColorSpinorField &y, const Exec &ex) { run<R_NONE>(a, x, 1.0, y, true, ex); }
       double norm2(const ColorSpinorField &x, const Exec &ex)
       {
@@ -1496,6 +1523,60 @@ namespace b200
         site(tmp, b_other, other_parity, true);
         hop(src, tmp, this_parity, Fuse::None, &b_this, kappa);
       }
+    }
+
+    // ---- clover force (lib/clover_force.cpp)
+    void computeCloverForce(void *mom, double dt, const std::vector<ColorSpinorField> &x, const double *coeff, double kappa2,
+                            double ck, double multiplicity, const void *const qdp[4], const void *packed, const Dirac &op)
+    {
+      if (!op.is_clover() || !op.pc()) throw Error("the clover force needs an even-odd preconditioned clover operator");
+      if (op.is_symmetric()) throw Error("the clover force needs asymmetric preconditioning (EVEN_EVEN_ASYMMETRIC or ODD_ODD_ASYMMETRIC)");
+      if (op.Comm() && op.Comm()->partitioned()) throw Error("the clover force runs on one GPU: the lattice must not be partitioned");
+      const int n = (int)x.size();
+      if (n < 1 || n > B200_MAX_SHIFTS) throw Error("the clover force takes 1 to " + std::to_string(B200_MAX_SHIFTS) + " solutions");
+      for (const auto &f : x)
+        if (f.n_parity != 1 || f.precision != op.Precision()) throw Error("each solution must be a single-parity field of the operator's precision");
+      const int par = op.thisParity(), oth = 1 - par;
+      const Exec ex = op.exec();
+      // p_i and the other parity of x_i, prepared along the dagger branch of the reference (gamma5, dagger Dslash of the
+      // other parity, Mhat^+, gamma5; then the plain Dslash): for solutions of (Mhat^+ Mhat + sigma) x = phi this is the
+      // derivative of phi^+ (Mhat^+ Mhat + sigma)^-1 phi.  That branch hands p to the outer products in x's place.
+      std::vector<std::unique_ptr<Scratch>> xf, pf;
+      std::vector<const void *> xp, pp;
+      Scratch t(op.Stream(), x[0], 1);
+      for (int i = 0; i < n; i++) {
+        xf.emplace_back(new Scratch(op.Stream(), x[i], 2));
+        pf.emplace_back(new Scratch(op.Stream(), x[i], 2));
+        ColorSpinorField &X = *xf.back(), &P = *pf.back();
+        auto x_oth = X.parity_view(oth), x_par = X.parity_view(par), p_par = P.parity_view(par), p_oth = P.parity_view(oth);
+        blas::gamma5(t, x[i], ex);
+        op.flipDagger();
+        try {
+          op.Dslash(x_oth, t, oth);
+          op.M(p_par, t);
+        } catch (...) {
+          op.flipDagger();
+          throw;
+        }
+        op.flipDagger();
+        blas::gamma5(x_oth, x_oth, ex);
+        op.Dslash(p_oth, p_par, oth);
+        blas::gamma5(P, P, ex);
+        blas::copy(x_par, x[i], ex);
+        xp.push_back(P.v);
+        pp.push_back(X.v);
+      }
+      std::vector<double> fc(n), eps(2 * (size_t)n);
+      for (int i = 0; i < n; i++) {
+        fc[i] = 2.0 * dt * coeff[i] * kappa2;
+        // the reference indexes epsilon by site parity; its first entry belongs to the matpc parity
+        eps[2 * i + par] = 2.0 * ck * coeff[i] * dt;
+        eps[2 * i + oth] = -kappa2 * 2.0 * ck * coeff[i] * dt;
+      }
+      const GaugeField &U = op.Gauge();
+      abi_ok(b200_clover_force_accumulate(mom, qdp, packed, U.X, op.Precision(), n, xp.data(), pp.data(), fc.data(), eps.data(),
+                                          2.0 * ck * multiplicity * dt, oth, op.Stream()));
+      cuda_ok(cudaStreamSynchronize(cs(op.Stream())), "clover force");
     }
 
     // x_o = A_o^-1 (b_o + k D_oe x_e)

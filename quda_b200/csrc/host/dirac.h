@@ -140,6 +140,7 @@ namespace b200
     {
       void copy(ColorSpinorField &dst, const ColorSpinorField &src, const Exec &ex); // precision conversion allowed (8 <-> 4)
       void zero(ColorSpinorField &x, const Exec &ex);
+      void gamma5(ColorSpinorField &out, const ColorSpinorField &in, const Exec &ex); // UKQCD basis, in place allowed (8 / 4)
       void axpy(double a, const ColorSpinorField &x, ColorSpinorField &y, const Exec &ex); // y += a x
       // the reductions below synchronise the stream (they return the global sum to the host)
       double norm2(const ColorSpinorField &x, const Exec &ex);
@@ -198,6 +199,10 @@ namespace b200
 
       bool pc() const { return schur; }
       bool is_twisted() const { return term == SiteTerm::Twist; }
+      bool is_clover() const { return term == SiteTerm::Clover; }
+      bool is_symmetric() const { return symmetric; }
+      int thisParity() const { return this_parity; }
+      const GaugeField &Gauge() const { return *gauge; }
       void setMu(double m) { mu = m; }
       void setCommDim(const int *c) { for (int d = 0; d < 4; d++) commDim[d] = c[d]; }
       void flipDagger() const { dagger = !dagger; }
@@ -253,6 +258,13 @@ namespace b200
     // Solve (MdagM + offset[j]) x_j = b for j < n_shift; x holds n_shift fields, which are overwritten
     void invertMultiShiftCG(const Dirac &mat, const Dirac &matSloppy, std::vector<ColorSpinorField> &x, const ColorSpinorField &b,
                             MultiShiftParam &param);
+
+    // ---- clover fermion force of the pseudofermion action sum_i coeff_i phi^+ (Mhat^+ Mhat + sigma_i)^-1 phi and of
+    // -multiplicity tr log A on the other parity (computeCloverForceQuda, lib/clover_force.cpp): x holds the solutions on
+    // the operator's parity; mom [V][4][10] is updated by b200_clover_force_accumulate.  Needs an asymmetric "cloverpc"
+    // operator on an unpartitioned lattice; synchronises the operator's stream.
+    void computeCloverForce(void *mom, double dt, const std::vector<ColorSpinorField> &x, const double *coeff, double kappa2,
+                            double ck, double multiplicity, const void *const qdp[4], const void *packed, const Dirac &op);
 
     // true if a halo wait gave up since the last call (clears the flag); the C entry points turn it into an error
     bool halo_timed_out(CommContext *comm, void *stream);

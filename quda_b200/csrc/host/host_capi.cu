@@ -280,4 +280,24 @@ int b200_invert_multishift_cg(b200_dirac *precise, b200_dirac *sloppy, const b20
     param->host_syncs = mp.host_syncs;
   });
 }
+
+int b200_clover_force(void *mom, double dt, const b200_spinor *x, const double *coeff, double kappa2, double ck, int n,
+                      double multiplicity, const void *const qdp[4], const void *packed, b200_dirac *op)
+{
+  const char *name = "b200_clover_force";
+  if (!mom || !x || !coeff || !qdp || !packed || !op) return b200::set_error(B200_ERR_INVALID, "%s: null argument", name);
+  if (n < 1 || n > B200_MAX_SHIFTS) return b200::set_error(B200_ERR_INVALID, "%s: n=%d not in [1, %d]", name, n, B200_MAX_SHIFTS);
+  const Dirac &d = *op->op;
+  if (!d.is_clover() || !d.pc() || d.is_symmetric() || (op->has_comm && op->user_comm && [&] {
+        pull_comm(op);
+        return op->comm.partitioned();
+      }()))
+    return b200::set_error(B200_ERR_INVALID, "%s: needs an asymmetric \"cloverpc\" operator on an unpartitioned lattice", name);
+  if (int rc = b200::require_device()) return rc;
+  return guarded([&] {
+    std::vector<ColorSpinorField> xs;
+    for (int i = 0; i < n; i++) xs.push_back(wrap(op, &x[i]));
+    computeCloverForce(mom, dt, xs, coeff, kappa2, ck, multiplicity, qdp, packed, d);
+  });
+}
 }

@@ -128,3 +128,36 @@ def invert_multishift_cg(precise, sloppy, xs, b, offsets, tol=1e-10, tol_offset=
     L.check(precise.lib.b200_invert_multishift_cg(precise.h, sloppy.h if sloppy is not None else None, xd, C.byref(bd),
                                                   C.byref(p)))
     return p
+
+
+def compute_clover_force(mom, dt, xs, coeffs, kappa, csw, multiplicity, gauge, op):
+    """computeCloverForceQuda: add to mom ([V][4][10] device tensor of the operator's precision, parity-major sites; per link
+    the (01), (02), (12) complex entries, the three imaginary diagonals and one pad real) the clover fermion force of
+    sum_j coeffs[j] phi^+ (Mhat^+ Mhat + sigma_j)^-1 phi - multiplicity tr log A_other, dt times over.  xs are the solutions
+    invert_multishift_cg wrote, gauge the QDP-order links given to compute_clover_field (boundary signs included), op an
+    asymmetric "cloverpc" Dirac (fp64 or fp32) on one GPU.  The packed A is rebuilt from gauge with dslash.compute_clover.
+    (kappa, csw) become the reference's kappa2 = -kappa^2 and ck = -csw kappa / 8, the convention MILC passes; with them
+    the update is the derivative of the action above for A = 1 + kappa csw sum sigma F as compute_clover_field builds it."""
+    import torch
+
+    from . import dslash as D
+    from . import fields as F
+    n = len(xs)
+    if not 1 <= n <= L.MAX_SHIFTS or len(coeffs) != n:
+        raise L.B200Error(f"compute_clover_force: {n} solutions and {len(coeffs)} coefficients, 1 to {L.MAX_SHIFTS} pairs")
+    if op.prec not in (F.DOUBLE, F.SINGLE):
+        raise L.B200Error(f"compute_clover_force: operator precision {op.prec}, the force runs in fp64 or fp32")
+    _need_precise("compute_clover_force", op, [(f"x[{j}]", x) for j, x in enumerate(xs)])
+    dt_ = torch.float64 if op.prec == F.DOUBLE else torch.float32
+    X = op.U.X
+    if mom.dtype != dt_ or tuple(mom.shape) != (2 * F.volume_cb(X), 4, 10) or not mom.is_contiguous():
+        raise L.B200Error(f"compute_clover_force: mom must be a contiguous {dt_} tensor of shape [V][4][10]")
+    g = torch.as_tensor(gauge).to(device="cuda", dtype=dt_).contiguous()
+    packed = torch.empty((2 * F.volume_cb(X), 2, 36), dtype=dt_, device="cuda")
+    D.compute_clover(packed, g, X, [0, 0, 0, 0], op.prec, kappa * csw)
+    torch.cuda.synchronize()
+    q = (C.c_void_p * 4)(*[g[mu].data_ptr() for mu in range(4)])
+    xd = (L.Spinor * n)(*[x.desc() for x in xs])
+    cd = (C.c_double * n)(*[float(c) for c in coeffs])
+    L.check(op.lib.b200_clover_force(mom.data_ptr(), float(dt), xd, cd, -kappa * kappa, -csw * kappa / 8.0, n,
+                                     float(multiplicity), q, packed.data_ptr(), op.h))

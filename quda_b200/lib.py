@@ -131,6 +131,17 @@ def declare_clover(lib, prefix="b200"):
     return lib
 
 
+def declare_clover_force(lib, prefix="b200"):
+    """Attach argtypes/restypes for the kernel-level clover force, shared by the CUDA library and its test-only twin."""
+    f = getattr(lib, prefix + "_clover_force_accumulate")
+    f.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.POINTER(C.c_int), C.c_int, C.c_int, C.POINTER(C.c_void_p),
+                  C.POINTER(C.c_void_p), C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_double, C.c_int, C.c_void_p]
+    f.restype = C.c_int
+    f = getattr(lib, prefix + "_last_error")
+    f.argtypes, f.restype = [], C.c_char_p
+    return lib
+
+
 _lib = None
 
 
@@ -143,6 +154,7 @@ def load():
         lib = C.CDLL(LIB_PATH)
         declare(lib)
         declare_clover(lib)
+        declare_clover_force(lib)
         lib.b200_abi_version.restype = C.c_int
         lib.b200_launch_count.restype = C.c_long
         lib.b200_ghost_face_bytes.argtypes = [C.c_int, C.POINTER(C.c_int), C.c_int]
@@ -182,6 +194,9 @@ def load():
         lib.b200_invert_multishift_cg.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(Spinor), C.POINTER(Spinor),
                                                   C.POINTER(MultiShiftParam)]
         lib.b200_invert_multishift_cg.restype = C.c_int
+        lib.b200_clover_force.argtypes = [C.c_void_p, C.c_double, C.POINTER(Spinor), C.POINTER(C.c_double), C.c_double,
+                                          C.c_double, C.c_int, C.c_double, C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p]
+        lib.b200_clover_force.restype = C.c_int
         lib.b200_comm_check.argtypes, lib.b200_comm_check.restype = [C.POINTER(Comm), C.c_void_p], C.c_int
         if lib.b200_abi_version() != ABI_VERSION:
             raise B200Error("libquda_b200.so ABI version mismatch")
@@ -197,7 +212,8 @@ def check(rc, lib=None, prefix="b200"):
 
 
 EXPORTED_SYMBOLS = ["b200_dslash_apply", "b200_dslash_apply_fused", "b200_dslash_apply_multi", "b200_clover_apply", "b200_twist_gamma5", "b200_pack_ghost", "b200_pack_ghost_multi", "b200_ghost_face_bytes",
-                    "b200_copy_spinor", "b200_copy_gauge", "b200_copy_clover", "b200_compute_clover", "b200_clover_invert_packed", "b200_comm_alloc", "b200_comm_free", "b200_ipc_get_handle", "b200_ipc_open_handle",
+                    "b200_copy_spinor", "b200_copy_gauge", "b200_copy_clover", "b200_compute_clover", "b200_clover_invert_packed",
+                    "b200_clover_force_accumulate", "b200_clover_force", "b200_comm_alloc", "b200_comm_free", "b200_ipc_get_handle", "b200_ipc_open_handle",
                     "b200_ipc_close_handle", "b200_comm_copy",
                     "b200_dirac_create", "b200_dirac_set_twist", "b200_dirac_destroy", "b200_dirac_apply", "b200_dirac_prepare",
                     "b200_dirac_reconstruct", "b200_invert_cg", "b200_invert_bicgstab", "b200_invert_multishift_cg",
