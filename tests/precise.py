@@ -500,9 +500,8 @@ def _site_matrix(blocks, prec, scale=1.0):
     return blocks.real.dtype.type(scale) * (KN @ Hbd @ KR), KN, Hbd, KR
 
 
-def hermitian_inverse(H):
-    """inverse of Hermitian positive-definite blocks [..., 6, 6] by Cholesky, in the blocks' own precision
-    (np.linalg has no long double)"""
+def cholesky(H):
+    """lower Cholesky factor of Hermitian positive-definite blocks [..., n, n], in the blocks' own precision"""
     n = H.shape[-1]
     L = np.zeros_like(H)
     for j in range(n):
@@ -510,6 +509,14 @@ def hermitian_inverse(H):
         L[..., j, j] = np.sqrt(d)
         for i in range(j + 1, n):
             L[..., i, j] = (H[..., i, j] - np.sum(L[..., i, :j] * np.conj(L[..., j, :j]), axis=-1)) / L[..., j, j]
+    return L
+
+
+def hermitian_inverse(H):
+    """inverse of Hermitian positive-definite blocks [..., 6, 6] by Cholesky, in the blocks' own precision
+    (np.linalg has no long double)"""
+    n = H.shape[-1]
+    L = cholesky(H)
     Linv = np.zeros_like(H)
     for i in range(n):
         Linv[..., i, i] = 1 / L[..., i, i]

@@ -60,7 +60,17 @@ def _solve(gauge, X, phi, matpc, U=None):
 
 @pytest.mark.parametrize("matpc", [DR.MATPC_EVEN_EVEN_ASYMMETRIC, DR.MATPC_ODD_ODD_ASYMMETRIC])
 def test_pipeline_matches_restatement(matpc):
-    X, dt, mult = (8, 8, 8, 8), 0.25, 2
+    _pipeline((8, 8, 8, 8), matpc)
+
+
+@pytest.mark.parametrize("matpc", [DR.MATPC_EVEN_EVEN_ASYMMETRIC, DR.MATPC_ODD_ODD_ASYMMETRIC])
+def test_pipeline_matches_restatement_non_hypercubic(matpc):
+    """all four extents distinct: a dimension mix-up anywhere in the pipeline shows"""
+    _pipeline((4, 6, 8, 10), matpc)
+
+
+def _pipeline(X, matpc):
+    dt, mult = 0.25, 2
     gauge = oracle.random_gauge(X, 8, seed=41, antiperiodic_t=True)
     phi = oracle.random_spinor(X, 8, seed=43) - 0.5
     xs, _, op, P = _solve(gauge, X, phi, matpc)
