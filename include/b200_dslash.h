@@ -392,6 +392,35 @@ int b200_clover_force_accumulate(void *mom, const void *const qdp[4], const void
 int b200_clover_force(void *mom, double dt, const b200_spinor *x, const double *coeff, double kappa2, double ck, int n,
                       double multiplicity, const void *const qdp[4], const void *packed, b200_dirac *op);
 
+/* The gauge half of an HMC step on one GPU (no partitioned dimension): computeGaugeForceQuda, updateGaugeFieldQuda,
+ * momActionQuda and plaqQuda (lib/interface_quda.cpp).  Fields as for the clover force: qdp[mu] are device QDP-order links
+ * [V][3][3][2] with the fermion boundary sign included (every closed loop crosses the t boundary an even number of times,
+ * so the sign cancels in the force and the plaquette, and exp(dt P)(-U) = -exp(dt P) U keeps it through the update); mom is
+ * [V][4][10] as above.  Sites are parity-major, neighbours wrap periodically.  precision is 8 or 4 for every field.
+ *
+ * Gauge force: for every link U_mu(x),
+ *   mom <- TA(mom - eb3 U_mu(x) sum_i coeff[i] path_i),
+ * path_i the ordered product of the links of paths[mu][i][0 .. length[i]) (steps 0..3 forward along that direction, 7 - d
+ * backward along d) walked from x + mu-hat; it must end at x.  paths is a flat int array [4][num_paths][max_length];
+ * length and coeff have num_paths entries.  The path table travels in the kernel's parameter block, which bounds it:
+ * 1 <= num_paths <= B200_GAUGE_MAX_PATHS, 1 <= length[i] <= max_length <= B200_GAUGE_MAX_LENGTH.  Steps outside 0..7
+ * and open paths are refused.  Asynchronous on `stream`. */
+#define B200_GAUGE_MAX_PATHS 64  /* the Symanzik set (plaquette, rectangle and parallelogram staples) has 48 */
+#define B200_GAUGE_MAX_LENGTH 12 /* steps per path after the first link U_mu(x) */
+int b200_gauge_force(void *mom, const void *const qdp[4], const int X[4], int precision, const int *paths, const int *length,
+                     const double *coeff, int num_paths, int max_length, double eb3, void *stream);
+/* out[mu] = exp(dt P) in[mu] for every link, P the traceless part of mom (conj_mom: of its adjoint).  exact = 1: the closed
+ * form of the SU(3) exponential (Cayley-Hamilton, Morningstar & Peardon hep-lat/0311018); exact = 0: the order-8 Taylor
+ * expansion of the reference (Horner form).  out may be in.  Asynchronous on `stream`. */
+int b200_update_gauge(void *const out[4], const void *const in[4], const void *mom, const int X[4], int precision, double dt,
+                      int conj_mom, int exact, void *stream);
+/* *S = sum over links of 1/2 sum_k (Im P_kk)^2 + sum_{i<j} |P_ij|^2 - 4 (MILC's normalisation), summed in double in a
+ * fixed order: repeated calls give identical sums.  Synchronises `stream`. */
+int b200_mom_action(double *S, const void *mom, const int X[4], int precision, void *stream);
+/* plaq = {total, spatial, temporal}: the mean of Re tr P_mu,nu / 3 over the sites and the three spatial (mu, nu < 3),
+ * resp. temporal planes; total = (spatial + temporal) / 2.  Fixed-order double sums; synchronises `stream`. */
+int b200_plaquette(double plaq[3], const void *const qdp[4], const int X[4], int precision, void *stream);
+
 const char *b200_last_error(void);
 int b200_abi_version(void);
 /* number of kernels this library has launched since load (bench.py's gpu_launches evidence) */

@@ -6,6 +6,7 @@
 
 #include "clover_build.h"
 #include "clover_force.h"
+#include "gauge.h"
 #include "plan.h"
 
 namespace b200
@@ -55,6 +56,10 @@ namespace b200
     template <typename T> static int clover_build(const CloverBuildRequest &rq) { return launch_clover_build<T>(rq); }
     template <typename T> static int clover_invert(const CloverInvertRequest &rq) { return launch_clover_invert<T>(rq); }
     template <typename T> static int clover_force(const CloverForceRequest &rq) { return launch_clover_force<T>(rq); }
+    template <typename T> static int gauge_force(const GaugeForceRequest &rq) { return launch_gauge_force<T>(rq); }
+    template <typename T> static int gauge_update(const GaugeUpdateRequest &rq) { return launch_gauge_update<T>(rq); }
+    template <typename T> static int mom_action(const GaugeSumRequest &rq, double g[2]) { return launch_mom_action<T>(rq, g); }
+    template <typename T> static int plaquette(const GaugeSumRequest &rq, double g[4]) { return launch_plaquette<T>(rq, g); }
   };
 
 } // namespace b200
@@ -184,6 +189,28 @@ int b200_clover_force_accumulate(void *mom, const void *const qdp[4], const void
                                  double sigma_coeff, int trlog_parity, void *stream)
 {
   return clover_force_accumulate<Cuda>(mom, qdp, packed, X, precision, n, x, p, force_coeff, epsilon, sigma_coeff, trlog_parity, stream);
+}
+
+int b200_gauge_force(void *mom, const void *const qdp[4], const int X[4], int precision, const int *paths, const int *length,
+                     const double *coeff, int num_paths, int max_length, double eb3, void *stream)
+{
+  return gauge_force<Cuda>(mom, qdp, X, precision, paths, length, coeff, num_paths, max_length, eb3, stream);
+}
+
+int b200_update_gauge(void *const out[4], const void *const in[4], const void *mom, const int X[4], int precision, double dt,
+                      int conj_mom, int exact, void *stream)
+{
+  return update_gauge<Cuda>(out, in, mom, X, precision, dt, conj_mom, exact, stream);
+}
+
+int b200_mom_action(double *S, const void *mom, const int X[4], int precision, void *stream)
+{
+  return mom_action<Cuda>(S, mom, X, precision, stream);
+}
+
+int b200_plaquette(double plaq[3], const void *const qdp[4], const int X[4], int precision, void *stream)
+{
+  return plaquette<Cuda>(plaq, qdp, X, precision, stream);
 }
 
 int b200_comm_alloc(void **ptr, size_t bytes)

@@ -256,16 +256,24 @@ def copy_spinor(native, host_order, to_native, stream=None):
 
 def load_gauge(host_gauge, X, prec, recon, anisotropy=1.0, t_boundary=1, ghost_links=None, first_time_slice=True,
                last_time_slice=True, stream=None):
-    """loadGaugeQuda's device work: host QDP-order gauge (numpy [4][V][3][3][2], fp64/fp32) -> resident native GaugeField
-    at (`prec`, `recon`) with the pad filled (ghost_links[mu]: neighbour's boundary links, None = periodic self).
+    """loadGaugeQuda's device work: QDP-order gauge ([4][V][3][3][2], fp64/fp32: a host numpy array, or a CUDA tensor such
+    as gauge.update_gauge_field returns, used where it lies) -> resident native GaugeField at (`prec`, `recon`) with the pad
+    filled (ghost_links[mu]: neighbour's boundary links, None = periodic self).
     Reference: lib/interface_quda.cpp:571-764, lib/copy_gauge*.cu, lib/extract_gauge_ghost*."""
     import torch
     lib = L.load()
     Vh = F.volume_cb(X)
     pad = F.gauge_pad(X)
     stride = Vh + pad
-    h = torch.from_numpy(np.ascontiguousarray(host_gauge)).cuda()
-    link_max = float(np.abs(host_gauge).max())
+    if isinstance(host_gauge, torch.Tensor):
+        if host_gauge.dtype not in (torch.float64, torch.float32):
+            raise L.B200Error("load_gauge: the links must be float64 or float32")
+        h = host_gauge.to(device="cuda").contiguous()
+        link_max = float(h.abs().max())
+    else:
+        h = torch.from_numpy(np.ascontiguousarray(host_gauge)).cuda()
+        link_max = float(np.abs(host_gauge).max())
+    itemsize = h.element_size()
     nbytes = 2 * 4 * recon * stride * prec
     buf = torch.zeros(nbytes, dtype=torch.uint8, device="cuda")
     meta = dict(stride=stride, parity_stride_bytes=nbytes // 2, link_max=link_max, pad=pad)
@@ -278,12 +286,12 @@ def load_gauge(host_gauge, X, prec, recon, anisotropy=1.0, t_boundary=1, ghost_l
     gl = (C.c_void_p * 4)()
     for mu in range(4):
         if ghost_links is not None and ghost_links[mu] is not None:
-            t = torch.from_numpy(np.ascontiguousarray(ghost_links[mu]).astype(host_gauge.dtype)).cuda()
+            t = torch.from_numpy(np.ascontiguousarray(ghost_links[mu]).astype(np.float64 if itemsize == 8 else np.float32)).cuda()
             keep.append(t)
             gl[mu] = t.data_ptr()
         else:
             gl[mu] = None
-    L.check(lib.b200_copy_gauge(C.byref(d), prec, Xc, qdp, gl, host_gauge.dtype.itemsize, stream))
+    L.check(lib.b200_copy_gauge(C.byref(d), prec, Xc, qdp, gl, itemsize, stream))
     torch.cuda.synchronize()
     return U
 
