@@ -421,6 +421,26 @@ int b200_mom_action(double *S, const void *mom, const int X[4], int precision, v
  * resp. temporal planes; total = (spatial + temporal) / 2.  Fixed-order double sums; synchronises `stream`. */
 int b200_plaquette(double plaq[3], const void *const qdp[4], const int X[4], int precision, void *stream);
 
+/* The gradient flow of a gauge field (performWFlowQuda) and its clover observables (gaugeObservablesQuda), on one GPU with
+ * the fields of the gauge force above.
+ *
+ * Gradient flow: n_steps steps of Lüscher's RK3 integrator (arXiv:1006.4518, App. C) at step size epsilon (negative:
+ * the flow backwards) of dV/dt = Z(V) V with the generator Z_mu(x) = -TA(U_mu(x) sum_i coeff[i] path_i), the path table
+ * as for b200_gauge_force, so the flow follows the action sum_i coeff[i] sum_loops Re tr(1 - loop_i).  The plaquette
+ * staples with coeff 1 give the Wilson flow; plaquette 5/3 and rectangle -1/12 the Symanzik (Lüscher-Weisz) flow.  Every
+ * closed loop crosses the t boundary an even number of times and exp(Z)(-U) = -exp(Z) U, so the links keep the fermion
+ * boundary sign.  out may be in; in is otherwise left unchanged.  Scratch (one link field and [V][4][10]) is allocated
+ * and freed stream-ordered.  Asynchronous on `stream`. */
+int b200_gauge_flow(void *const out[4], const void *const in[4], const int X[4], int precision, const int *paths,
+                    const int *length, const double *coeff, int num_paths, int max_length, double epsilon, int n_steps,
+                    void *stream);
+/* From the clover F_mu,nu = (Q - Q^+) / 8 of the six planes (10, 20, 21, 30, 31, 32): energy = {total, spatial, temporal},
+ * spatial and temporal the sums over the sites and the planes with mu < 3, resp. mu = 3, of -Re tr(F^2) (F without its
+ * trace) over V; *qcharge = sum_x q(x), q(x) = -1/(4 pi^2) Re (tr F10 F32 - tr F20 F31 + tr F21 F30), written to the
+ * device array density[V] (parity-major; NULL: not written).  Fixed-order double sums; synchronises `stream`. */
+int b200_gauge_observables(double energy[3], double *qcharge, double *density, const void *const qdp[4], const int X[4],
+                           int precision, void *stream);
+
 const char *b200_last_error(void);
 int b200_abi_version(void);
 /* number of kernels this library has launched since load (bench.py's gpu_launches evidence) */

@@ -7,6 +7,7 @@
 #include "clover_build.h"
 #include "clover_force.h"
 #include "gauge.h"
+#include "gauge_flow.h"
 #include "plan.h"
 
 namespace b200
@@ -60,6 +61,8 @@ namespace b200
     template <typename T> static int gauge_update(const GaugeUpdateRequest &rq) { return launch_gauge_update<T>(rq); }
     template <typename T> static int mom_action(const GaugeSumRequest &rq, double g[2]) { return launch_mom_action<T>(rq, g); }
     template <typename T> static int plaquette(const GaugeSumRequest &rq, double g[4]) { return launch_plaquette<T>(rq, g); }
+    template <typename T> static int gauge_flow(const GaugeFlowRequest &rq) { return launch_gauge_flow<T>(rq); }
+    template <typename T> static int gauge_observables(const GaugeObsRequest &rq, double g[6]) { return launch_gauge_observables<T>(rq, g); }
   };
 
 } // namespace b200
@@ -211,6 +214,19 @@ int b200_mom_action(double *S, const void *mom, const int X[4], int precision, v
 int b200_plaquette(double plaq[3], const void *const qdp[4], const int X[4], int precision, void *stream)
 {
   return plaquette<Cuda>(plaq, qdp, X, precision, stream);
+}
+
+int b200_gauge_flow(void *const out[4], const void *const in[4], const int X[4], int precision, const int *paths,
+                    const int *length, const double *coeff, int num_paths, int max_length, double epsilon, int n_steps,
+                    void *stream)
+{
+  return gauge_flow<Cuda>(out, in, X, precision, paths, length, coeff, num_paths, max_length, epsilon, n_steps, stream);
+}
+
+int b200_gauge_observables(double energy[3], double *qcharge, double *density, const void *const qdp[4], const int X[4],
+                           int precision, void *stream)
+{
+  return gauge_observables<Cuda>(energy, qcharge, density, qdp, X, precision, stream);
 }
 
 int b200_comm_alloc(void **ptr, size_t bytes)

@@ -64,18 +64,16 @@ namespace b200
     return 0;
   }
 
-  inline int check_gauge_force(const void *mom, const void *const qdp[4], const int X[4], int precision, const int *paths,
-                               const int *length, const double *coeff, int num_paths, int max_length, double eb3)
+  // the path table of b200_gauge_force / b200_gauge_flow: sizes within the parameter block, finite coefficients, steps in
+  // 0..7, every path closed
+  inline int check_gauge_paths(const char *fn, const int *paths, const int *length, const double *coeff, int num_paths,
+                               int max_length)
   {
-    const char *fn = "b200_gauge_force";
-    if (!mom || !paths || !length || !coeff) return set_error(B200_ERR_INVALID, "%s: null argument", fn);
-    if (int rc = check_links(fn, qdp)) return rc;
-    if (int rc = check_clover_lattice(fn, X, precision)) return rc;
+    if (!paths || !length || !coeff) return set_error(B200_ERR_INVALID, "%s: null argument", fn);
     if (num_paths < 1 || num_paths > B200_GAUGE_MAX_PATHS)
       return set_error(B200_ERR_INVALID, "%s: num_paths=%d not in [1, %d]", fn, num_paths, B200_GAUGE_MAX_PATHS);
     if (max_length < 1 || max_length > B200_GAUGE_MAX_LENGTH)
       return set_error(B200_ERR_INVALID, "%s: max_length=%d not in [1, %d]", fn, max_length, B200_GAUGE_MAX_LENGTH);
-    if (!std::isfinite(eb3)) return set_error(B200_ERR_INVALID, "%s: eb3 is not finite", fn);
     for (int i = 0; i < num_paths; i++) {
       if (length[i] < 1 || length[i] > max_length)
         return set_error(B200_ERR_INVALID, "%s: length[%d]=%d not in [1, max_length=%d]", fn, i, length[i], max_length);
@@ -97,6 +95,18 @@ namespace b200
                            disp[0], disp[1], disp[2], disp[3]);
       }
     }
+    return 0;
+  }
+
+  inline int check_gauge_force(const void *mom, const void *const qdp[4], const int X[4], int precision, const int *paths,
+                               const int *length, const double *coeff, int num_paths, int max_length, double eb3)
+  {
+    const char *fn = "b200_gauge_force";
+    if (!mom) return set_error(B200_ERR_INVALID, "%s: null argument", fn);
+    if (int rc = check_links(fn, qdp)) return rc;
+    if (int rc = check_clover_lattice(fn, X, precision)) return rc;
+    if (int rc = check_gauge_paths(fn, paths, length, coeff, num_paths, max_length)) return rc;
+    if (!std::isfinite(eb3)) return set_error(B200_ERR_INVALID, "%s: eb3 is not finite", fn);
     return 0;
   }
 
@@ -193,12 +203,10 @@ namespace b200
     return mom + (((size_t)parity * volume_cb + x_cb) * 4 + mu) * 10;
   }
 
-  template <typename T> B2_HD void gauge_force_site(const GaugeForceArgs<T> &a, int x_cb, int parity, int mu)
+  // f = eb3 U_mu(x) sum_i c_i path_i(x) at coordinates y: the product the gauge force and the gradient flow (gauge_flow.h)
+  // project
+  template <typename T> B2_HD void gauge_path_sum(T *f, const GaugeForceArgs<T> &a, const int *y, int mu)
   {
-    Geom geo;
-    geom_init(geo, a.g.X);
-    int y[4];
-    coords_from_cb(y, geo, x_cb, parity);
     T s[18];
 #pragma unroll
     for (int k = 0; k < 18; k++) s[k] = 0;
@@ -234,11 +242,21 @@ namespace b200
 #pragma unroll
       for (int k = 0; k < 18; k++) s[k] = fma_rn(c, m[k], s[k]);
     }
-    T u[18], f[18];
+    T u[18];
     load_link_ext(u, a.g, mu, y, 0, 0, 0, 0);
     su3_mul_op<false, false>(f, u, s);
 #pragma unroll
     for (int k = 0; k < 18; k++) f[k] = mul_rn(a.eb3, f[k]);
+  }
+
+  template <typename T> B2_HD void gauge_force_site(const GaugeForceArgs<T> &a, int x_cb, int parity, int mu)
+  {
+    Geom geo;
+    geom_init(geo, a.g.X);
+    int y[4];
+    coords_from_cb(y, geo, x_cb, parity);
+    T f[18];
+    gauge_path_sum(f, a, y, mu);
     mom_sub_ta(mom_at(a.mom, a.g.volume_cb, x_cb, parity, mu), f);
   }
 

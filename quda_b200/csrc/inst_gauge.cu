@@ -82,7 +82,8 @@ namespace b200
   }
 
   // the second stage and the copy of the `groups` sums to the host, then the scratch is freed and the stream synchronised
-  static int finish_sums(double *scratch, int nblk, int groups, double *g, cudaStream_t s)
+  // (also the last step of inst_gauge_flow.cu's observables)
+  int finish_sums(double *scratch, int nblk, int groups, double *g, cudaStream_t s)
   {
     clover_trlog_kernel<<<groups, kGaugeThreads, 0, s>>>(scratch, nblk, scratch + (size_t)groups * nblk);
     count_launch();

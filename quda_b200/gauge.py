@@ -1,5 +1,6 @@
 """The gauge half of an HMC step on one GPU: computeGaugeForceQuda, updateGaugeFieldQuda, momActionQuda and plaqQuda
-(lib/interface_quda.cpp) on device tensors.
+(lib/interface_quda.cpp) on device tensors; and the measurement that follows a trajectory: the Wilson and Symanzik
+gradient flow with the clover energy density and topological charge along it (performWFlowQuda, gaugeObservablesQuda).
 
 Field orders, shared with dslash.compute_clover_field and dirac.compute_clover_force:
   gauge  [4][V][3][3][2] QDP-order links (fp64 or fp32), parity-major sites, fermion boundary sign included -- every closed
@@ -116,3 +117,111 @@ def plaquette(gauge, *, X, stream=None, backend=None):
     p = (C.c_double * 3)()
     L.check(getattr(lib, prefix + "_plaquette")(p, _links(gauge), _lattice(X), prec, stream), lib, prefix)
     return tuple(p)
+
+
+# ------------------------------------------------------------------ gradient flow
+def _enc(step):
+    """signed step +-(d + 1) -> the path code: d forward, 7 - d backward"""
+    return step - 1 if step > 0 else 7 + step + 1
+
+
+def _loops_to_paths(loops):
+    return [[_enc(s) for s in loop[1:]] for loop in loops]
+
+
+def _plaquettes(mu):
+    return [[mu + 1, s * (nu + 1), -(mu + 1), -s * (nu + 1)] for nu in range(4) if nu != mu for s in (1, -1)]
+
+
+def _rectangles(mu):
+    out = []
+    for nu in range(4):
+        if nu == mu:
+            continue
+        for s in (1, -1):
+            m, n = mu + 1, s * (nu + 1)
+            out += [[m, m, n, -m, -m, -n], [m, n, -m, -m, -n, m], [m, n, n, -m, -n, -n]]  # each 2x1 loop through the link once
+    return out
+
+
+def _action(kinds):
+    paths = [sum((_loops_to_paths(k(mu)) for k, _ in kinds), []) for mu in range(4)]
+    coeffs = sum(([c] * len(k(0)) for k, c in kinds), [])
+    return paths, coeffs
+
+
+# name -> (paths[mu][i], coeffs) of the flow action sum_i c_i sum_loops Re tr(1 - loop_i): Wilson (the plaquette, c = 1)
+# and Symanzik / Luscher-Weisz (plaquette 5/3, rectangle -1/12), as in the reference's gauge_wilson_flow.cuh
+FLOW_ACTIONS = {"wilson": _action([(_plaquettes, 1.0)]),
+                "symanzik": _action([(_plaquettes, 5.0 / 3), (_rectangles, -1.0 / 12)])}
+
+
+def gauge_observables(gauge, *, X, density=None, stream=None, backend=None):
+    """gaugeObservablesQuda: {"plaquette": (total, spatial, temporal), "energy": (total, spatial, temporal), "qcharge": Q}.
+    energy is the clover E = -sum_planes Re tr(F^2) / V (F = (Q - Q^+) / 8 without its trace, spatial: the planes of two
+    spatial directions), Q = sum_x q(x) with q = -1/(4 pi^2) Re (tr F10 F32 - tr F20 F31 + tr F21 F30).  density, a float64
+    CUDA tensor of V elements, receives q(x) in parity-major site order."""
+    V = int(np.prod(_lattice(X)))
+    prec = _check_field("gauge", gauge, (4, V, 3, 3, 2))
+    dptr = None
+    if density is not None:
+        import torch
+        if (not isinstance(density, torch.Tensor) or not density.is_cuda or density.dtype != torch.float64
+                or density.numel() != V or not density.is_contiguous()):
+            raise L.B200Error(f"gauge_observables: density must be a contiguous float64 CUDA tensor of {V} elements")
+        dptr = density.data_ptr()
+    prefix, lib = backend or ("b200", L.load())
+    e, q = (C.c_double * 3)(), C.c_double()
+    L.check(getattr(lib, prefix + "_gauge_observables")(e, C.byref(q), dptr, _links(gauge), _lattice(X), prec, stream),
+            lib, prefix)
+    return {"plaquette": plaquette(gauge, X=X, stream=stream, backend=backend), "energy": tuple(e), "qcharge": q.value}
+
+
+def gauge_flow(out, gauge, epsilon, n_steps, paths, coeffs, *, X, stream=None, backend=None):
+    """n_steps RK3 steps of size epsilon of the gradient flow of the action sum_i coeffs[i] sum_loops Re tr(1 - loop_i),
+    the loops given as gauge_force paths, from gauge into out (out may be gauge)"""
+    V = int(np.prod(_lattice(X)))
+    prec = _check_field("gauge", gauge, (4, V, 3, 3, 2))
+    if _check_field("out", out, (4, V, 3, 3, 2)) != prec:
+        raise L.B200Error("gauge_flow: out must have the precision of gauge")
+    table, lengths, n, max_length = path_table(paths)
+    if len(coeffs) != n:
+        raise L.B200Error(f"gauge_flow: {n} paths and {len(coeffs)} coefficients")
+    prefix, lib = backend or ("b200", L.load())
+    L.check(getattr(lib, prefix + "_gauge_flow")(
+        _links(out), _links(gauge), _lattice(X), prec, table.ctypes.data_as(C.POINTER(C.c_int)), (C.c_int * n)(*lengths),
+        (C.c_double * n)(*[float(c) for c in coeffs]), n, max_length, float(epsilon), int(n_steps), stream), lib, prefix)
+    return out
+
+
+def gradient_flow(gauge, epsilon, n_steps, *, X, action="wilson", meas_interval=0, out=None, stream=None, backend=None):
+    """performWFlowQuda: flow gauge by n_steps RK3 steps of size epsilon (Luscher, arXiv:1006.4518) under the action
+    FLOW_ACTIONS[action].  Returns (flowed, rows); with meas_interval > 0 a row (t, plaquette, energy, qcharge) of
+    gauge_observables is taken at t = 0 and after every meas_interval steps.  out defaults to a new tensor; out=gauge flows
+    in place."""
+    import torch
+    if action not in FLOW_ACTIONS:
+        raise L.B200Error(f"gradient_flow: action {action!r} not in {sorted(FLOW_ACTIONS)}")
+    n_steps, meas_interval = int(n_steps), int(meas_interval)
+    if n_steps < 1 or meas_interval < 0:
+        raise L.B200Error("gradient_flow: n_steps must be positive and meas_interval non-negative")
+    paths, coeffs = FLOW_ACTIONS[action]
+    rows = []
+
+    def measure(g, step):
+        o = gauge_observables(g, X=X, stream=stream, backend=backend)
+        rows.append((step * float(epsilon), o["plaquette"], o["energy"], o["qcharge"]))
+
+    if meas_interval:
+        measure(gauge, 0)
+    if out is None:
+        out = torch.empty_like(gauge)
+    chunk = meas_interval or n_steps
+    src, done = gauge, 0
+    while done < n_steps:
+        k = min(chunk, n_steps - done)
+        gauge_flow(out, src, epsilon, k, paths, coeffs, X=X, stream=stream, backend=backend)
+        src, done = out, done + k
+        if meas_interval and k == meas_interval:
+            measure(out, done)
+    return out, rows
