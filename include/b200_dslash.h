@@ -441,6 +441,29 @@ int b200_gauge_flow(void *const out[4], const void *const in[4], const int X[4],
 int b200_gauge_observables(double energy[3], double *qcharge, double *density, const void *const qdp[4], const int X[4],
                            int precision, void *stream);
 
+/* Gauge smearing (performGaugeSmearQuda's four kinds), on one GPU with the fields of the gauge force above.  S_mu(x) is the
+ * sum of the staples of U_mu(x) over the smeared planes; d = 4, or 3 with 0 <= dir_ignore <= 3, which smears only the
+ * other three directions (their staples leave the ignored direction out) and copies the ignored direction's links bit for
+ * bit.  dir_ignore = -1 or 4: all four directions.  P[W] is the SU(3) projection: the unitary polar factor of W by Newton's
+ * iteration (to 2e-15 in fp64, 1e-6 in fp32, at most 100 iterations) over the principal cube root of its determinant.
+ *   B200_SMEAR_APE           coeff {alpha}:    U' = P[(1 - alpha) 1 + alpha / (2 (d - 1)) S U^+] U
+ *   B200_SMEAR_STOUT         coeff {rho}:      U' = exp(rho TA(S U^+)) U
+ *   B200_SMEAR_OVRIMP_STOUT  coeff {rho, eps}: the same with (5 - 2 eps) / 3 S - (1 - eps) / 12 R, R the 2x1 rectangle
+ *                                              staples (Moran & Leinweber, arXiv:0801.1165)
+ *   B200_SMEAR_HYP           coeff {alpha1, alpha2, alpha3}: Hasenfratz & Knechtli (hep-lat/0103029), every level
+ *                            P[(1 - alpha) 1 + c staples U^+] U; 4-d: alpha3 / 2, alpha2 / 4, alpha1 / 6; 3-d: alpha3 / 2,
+ *                            alpha2 / 4 (alpha1 unused)
+ * The projection of the product with U^+ and exp(X)(-U) = -exp(X) U keep the fermion boundary sign.  n_steps >= 1 steps;
+ * out may be in, which is otherwise unchanged.  Scratch is allocated and freed stream-ordered: the d smeared directions of
+ * one link field unless the call is one step out of place, plus for HYP the decorated links, 2 x 12 links per site in 4-d
+ * (3.6 GB at 32^4 in fp64) and 6 in 3-d.  Asynchronous on `stream`. */
+#define B200_SMEAR_APE 0
+#define B200_SMEAR_STOUT 1
+#define B200_SMEAR_OVRIMP_STOUT 2
+#define B200_SMEAR_HYP 3
+int b200_gauge_smear(void *const out[4], const void *const in[4], const int X[4], int precision, int type, const double coeff[3],
+                     int dir_ignore, int n_steps, void *stream);
+
 const char *b200_last_error(void);
 int b200_abi_version(void);
 /* number of kernels this library has launched since load (bench.py's gpu_launches evidence) */

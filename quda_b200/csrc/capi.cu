@@ -8,6 +8,7 @@
 #include "clover_force.h"
 #include "gauge.h"
 #include "gauge_flow.h"
+#include "gauge_smear.h"
 #include "plan.h"
 
 namespace b200
@@ -63,6 +64,7 @@ namespace b200
     template <typename T> static int plaquette(const GaugeSumRequest &rq, double g[4]) { return launch_plaquette<T>(rq, g); }
     template <typename T> static int gauge_flow(const GaugeFlowRequest &rq) { return launch_gauge_flow<T>(rq); }
     template <typename T> static int gauge_observables(const GaugeObsRequest &rq, double g[6]) { return launch_gauge_observables<T>(rq, g); }
+    template <typename T> static int gauge_smear(const GaugeSmearRequest &rq) { return launch_gauge_smear<T>(rq); }
   };
 
 } // namespace b200
@@ -227,6 +229,12 @@ int b200_gauge_observables(double energy[3], double *qcharge, double *density, c
                            int precision, void *stream)
 {
   return gauge_observables<Cuda>(energy, qcharge, density, qdp, X, precision, stream);
+}
+
+int b200_gauge_smear(void *const out[4], const void *const in[4], const int X[4], int precision, int type, const double coeff[3],
+                     int dir_ignore, int n_steps, void *stream)
+{
+  return gauge_smear<Cuda>(out, in, X, precision, type, coeff, dir_ignore, n_steps, stream);
 }
 
 int b200_comm_alloc(void **ptr, size_t bytes)

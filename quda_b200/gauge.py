@@ -1,6 +1,7 @@
 """The gauge half of an HMC step on one GPU: computeGaugeForceQuda, updateGaugeFieldQuda, momActionQuda and plaqQuda
 (lib/interface_quda.cpp) on device tensors; and the measurement that follows a trajectory: the Wilson and Symanzik
-gradient flow with the clover energy density and topological charge along it (performWFlowQuda, gaugeObservablesQuda).
+gradient flow with the clover energy density and topological charge along it (performWFlowQuda, gaugeObservablesQuda);
+and APE, stout, over-improved stout and HYP smearing (performGaugeSmearQuda).
 
 Field orders, shared with dslash.compute_clover_field and dirac.compute_clover_force:
   gauge  [4][V][3][3][2] QDP-order links (fp64 or fp32), parity-major sites, fermion boundary sign included -- every closed
@@ -221,6 +222,72 @@ def gradient_flow(gauge, epsilon, n_steps, *, X, action="wilson", meas_interval=
     while done < n_steps:
         k = min(chunk, n_steps - done)
         gauge_flow(out, src, epsilon, k, paths, coeffs, X=X, stream=stream, backend=backend)
+        src, done = out, done + k
+        if meas_interval and k == meas_interval:
+            measure(out, done)
+    return out, rows
+
+
+# ------------------------------------------------------------------ smearing
+# kind -> (B200_SMEAR_* code, the coefficient names of its coeff array, dir_ignore when none is given: performGaugeSmearQuda
+# smears APE and stout in 3-d with t ignored, over-improved stout and HYP in 4-d)
+SMEAR_KINDS = {"ape": (L.SMEAR_APE, ("alpha",), 3), "stout": (L.SMEAR_STOUT, ("rho",), 3),
+               "ovrimp_stout": (L.SMEAR_OVRIMP_STOUT, ("rho", "epsilon"), -1),
+               "hyp": (L.SMEAR_HYP, ("alpha1", "alpha2", "alpha3"), -1)}
+
+
+def _smear_kind(kind, dir_ignore):
+    if kind not in SMEAR_KINDS:
+        raise L.B200Error(f"smearing kind {kind!r} not in {sorted(SMEAR_KINDS)}")
+    code, names, default = SMEAR_KINDS[kind]
+    if dir_ignore is None or (int(dir_ignore) < 0 and code in (L.SMEAR_APE, L.SMEAR_STOUT)):
+        dir_ignore = default
+    return code, names, int(dir_ignore)
+
+
+def gauge_smear(out, gauge, kind, n_steps, *, X, alpha=0.0, rho=0.0, epsilon=0.0, alpha1=0.0, alpha2=0.0, alpha3=0.0,
+                dir_ignore=None, stream=None, backend=None):
+    """n_steps steps of smearing `kind` (SMEAR_KINDS) from gauge into out (out may be gauge).  APE takes alpha, stout rho,
+    over-improved stout rho and epsilon, HYP alpha1, alpha2, alpha3 (alpha1 unused in 3-d).  dir_ignore in 0..3 smears
+    only the other three directions and copies the ignored one; 4 smears all four.  None or a negative value is
+    performGaugeSmearQuda's default: t ignored for APE and stout, all four directions for over-improved stout and HYP."""
+    code, names, dir_ignore = _smear_kind(kind, dir_ignore)
+    V = int(np.prod(_lattice(X)))
+    prec = _check_field("gauge", gauge, (4, V, 3, 3, 2))
+    if _check_field("out", out, (4, V, 3, 3, 2)) != prec:
+        raise L.B200Error("gauge_smear: out must have the precision of gauge")
+    given = {"alpha": alpha, "rho": rho, "epsilon": epsilon, "alpha1": alpha1, "alpha2": alpha2, "alpha3": alpha3}
+    coeff = (C.c_double * 3)(*[float(given[n]) for n in names])
+    prefix, lib = backend or ("b200", L.load())
+    L.check(getattr(lib, prefix + "_gauge_smear")(_links(out), _links(gauge), _lattice(X), prec, code, coeff, dir_ignore,
+                                                  int(n_steps), stream), lib, prefix)
+    return out
+
+
+def smear(gauge, kind, n_steps, *, X, meas_interval=0, out=None, stream=None, backend=None, **coeffs):
+    """performGaugeSmearQuda: smear gauge by n_steps steps of `kind` with the coefficients and dir_ignore of gauge_smear.
+    Returns (smeared, rows); with meas_interval > 0 a row (step, plaquette, energy, qcharge) of gauge_observables is taken at
+    step 0 and after every meas_interval steps.  out defaults to a new tensor; out=gauge smears in place."""
+    import torch
+    _smear_kind(kind, coeffs.get("dir_ignore"))
+    n_steps, meas_interval = int(n_steps), int(meas_interval)
+    if n_steps < 1 or meas_interval < 0:
+        raise L.B200Error("smear: n_steps must be positive and meas_interval non-negative")
+    rows = []
+
+    def measure(g, step):
+        o = gauge_observables(g, X=X, stream=stream, backend=backend)
+        rows.append((step, o["plaquette"], o["energy"], o["qcharge"]))
+
+    if meas_interval:
+        measure(gauge, 0)
+    if out is None:
+        out = torch.empty_like(gauge)
+    chunk = meas_interval or n_steps
+    src, done = gauge, 0
+    while done < n_steps:
+        k = min(chunk, n_steps - done)
+        gauge_smear(out, src, kind, k, X=X, stream=stream, backend=backend, **coeffs)
         src, done = out, done + k
         if meas_interval and k == meas_interval:
             measure(out, done)

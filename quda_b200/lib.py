@@ -180,6 +180,18 @@ def declare_flow(lib, prefix="b200"):
     return lib
 
 
+def declare_smear(lib, prefix="b200"):
+    """Attach argtypes/restypes for gauge smearing, shared by the CUDA library and its test-only twin."""
+    P4 = C.POINTER(C.c_void_p)
+    f = getattr(lib, prefix + "_gauge_smear")
+    f.argtypes = [P4, P4, C.POINTER(C.c_int), C.c_int, C.c_int, C.POINTER(C.c_double), C.c_int, C.c_int, C.c_void_p]
+    f.restype = C.c_int
+    f = getattr(lib, prefix + "_last_error")
+    f.argtypes, f.restype = [], C.c_char_p
+    return lib
+
+
+SMEAR_APE, SMEAR_STOUT, SMEAR_OVRIMP_STOUT, SMEAR_HYP = 0, 1, 2, 3  # B200_SMEAR_*
 GAUGE_MAX_PATHS, GAUGE_MAX_LENGTH = 64, 12  # B200_GAUGE_MAX_PATHS, B200_GAUGE_MAX_LENGTH
 
 _lib = None
@@ -197,6 +209,7 @@ def load():
         declare_clover_force(lib)
         declare_gauge(lib)
         declare_flow(lib)
+        declare_smear(lib)
         lib.b200_abi_version.restype = C.c_int
         lib.b200_launch_count.restype = C.c_long
         lib.b200_ghost_face_bytes.argtypes = [C.c_int, C.POINTER(C.c_int), C.c_int]
@@ -256,7 +269,8 @@ def check(rc, lib=None, prefix="b200"):
 EXPORTED_SYMBOLS = ["b200_dslash_apply", "b200_dslash_apply_fused", "b200_dslash_apply_multi", "b200_clover_apply", "b200_twist_gamma5", "b200_pack_ghost", "b200_pack_ghost_multi", "b200_ghost_face_bytes",
                     "b200_copy_spinor", "b200_copy_gauge", "b200_copy_clover", "b200_compute_clover", "b200_clover_invert_packed",
                     "b200_clover_force_accumulate", "b200_clover_force", "b200_gauge_force", "b200_update_gauge",
-                    "b200_mom_action", "b200_plaquette", "b200_gauge_flow", "b200_gauge_observables", "b200_comm_alloc", "b200_comm_free", "b200_ipc_get_handle", "b200_ipc_open_handle",
+                    "b200_mom_action", "b200_plaquette", "b200_gauge_flow", "b200_gauge_observables", "b200_gauge_smear",
+                    "b200_comm_alloc", "b200_comm_free", "b200_ipc_get_handle", "b200_ipc_open_handle",
                     "b200_ipc_close_handle", "b200_comm_copy",
                     "b200_dirac_create", "b200_dirac_set_twist", "b200_dirac_destroy", "b200_dirac_apply", "b200_dirac_prepare",
                     "b200_dirac_reconstruct", "b200_invert_cg", "b200_invert_bicgstab", "b200_invert_multishift_cg",
